@@ -149,7 +149,9 @@ struct ScanArgs {
 	uint32_t cand_cap;
 	unsigned long long *cursor; // [0]: candidate slots reserved so far (in chunks: an upper bound of the candidates written)
 	uint32_t chunk;             // slots a warp reserves per atomicAdd
+	uint32_t *next_slice;       // zero at launch: slices taken from the shared counter so far (the kernel's dynamic schedule)
 	SegEntry *segs;
+	uint32_t *occ;  // one bit per segment, set with every entry written: the resolve reads only the entries whose bit is set
 	Cand *scratch;  // [gridDim.x * warps][slice bytes]: one private list per warp
 	uint32_t spt_shift;  // log2(slices per tile) = batch tile_shift - log2(Geom::kSlice)
 	uint32_t extra_smem; // bytes of engine-private shared memory behind the rings (hash table)

@@ -50,7 +50,10 @@ struct DevBuf {
 		if (p) cudaFree(p);
 		p = nullptr;
 		cap = 0;
-		size_t want = std::max<size_t>(n, 1024);
+		// a quarter of headroom: the buffers sized from the candidate slots a scan reserved vary a little from call to call
+		// (the scan's dynamic schedule decides which warp leaves how much of its last chunk unused), and a regrowth inside
+		// a call costs a device-wide cudaFree
+		size_t want = std::max<size_t>(n + n / 4, 1024);
 		cudaError_t e = cudaMalloc(&p, want * sizeof(T));
 		if (e == cudaSuccess) cap = want;
 		return e;
@@ -96,6 +99,7 @@ struct gscan_ctx {
 	gscan_stats stats;
 
 	DevBuf<SegEntry> segs;
+	DevBuf<uint32_t> occ;      // occupancy bits of segs, all zero between scans (k_gather clears what it read)
 	uint32_t seg_tag = 0;      // generation of the last scan that wrote segs (0: table freshly zeroed)
 	DevBuf<Cand> cand;
 	DevBuf<Cand> scratch;
@@ -107,7 +111,7 @@ struct gscan_ctx {
 	DevBuf<uint32_t> unit_start, unit_out, blk, chain, vm_flag, vm_unit_start;
 	DevBuf<OutRec> vm_ord;
 	DevBuf<unsigned long long> vm_budget;
-	DevBuf<unsigned long long> cursor; // [0] cursor, then 2 x u32 totals behind it
+	DevBuf<unsigned long long> cursor; // [0] cursor, [1..4] u32 totals (ResolveArgs::totals), [5] the scan's slice counter
 	DevBuf<uint8_t> pat_tables, hash_tables, vm_tables;
 	const uint32_t *vm_code = nullptr, *vm_sets = nullptr;
 	uint64_t pat_id = 0;
@@ -412,7 +416,7 @@ extern "C" void gscan_close(gscan_ctx *c)
 	if (c->job_active) { c->job.join(); c->job_active = false; }
 	cudaSetDevice(c->device);
 	cudaStreamSynchronize(c->stream);
-	c->segs.release(); c->cand.release(); c->scratch.release(); c->ord.release(); c->out.release();
+	c->segs.release(); c->occ.release(); c->cand.release(); c->scratch.release(); c->ord.release(); c->out.release();
 	c->unit_start.release(); c->unit_out.release(); c->blk.release(); c->chain.release(); c->vm_flag.release(); c->vm_unit_start.release(); c->vm_ord.release(); c->vm_budget.release(); c->cursor.release(); c->pat_tables.release(); c->hash_tables.release(); c->vm_tables.release();
 	c->probe_sum.release(); c->needle.release();
 	c->pool_arena.release(); c->pool_tiles.release(); c->pool_units.release();
@@ -702,7 +706,9 @@ static int ensure_segs(gscan_ctx *ctx, uint32_t n_segs)
 	const size_t before = ctx->segs.cap;
 	CK(ctx, ctx->segs.ensure(n_segs));
 	if (ctx->segs.cap != before || ctx->seg_tag >= 0xfffeu) {
+		CK(ctx, ctx->occ.ensure((ctx->segs.cap + 31) / 32));
 		CK(ctx, launch_fill_u32(reinterpret_cast<uint32_t *>(ctx->segs.p), ctx->segs.cap * 2, 0u, ctx->stream));
+		CK(ctx, launch_fill_u32(ctx->occ.p, ctx->occ.cap, 0u, ctx->stream));
 		ctx->seg_tag = 0;
 	}
 	ctx->seg_tag++;
@@ -829,7 +835,7 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 	const int grid = (int)std::min<uint32_t>((uint32_t)ctx->num_sms, b->n_tiles);
 	if (ensure_segs(ctx, n_segs) < 0) return -1;
 	CK(ctx, ctx->scratch.ensure((size_t)ctx->num_sms * geom.warps * geom.slice));
-	CK(ctx, ctx->cursor.ensure(2));
+	CK(ctx, ctx->cursor.ensure(6));
 	CK(ctx, ctx->readback.ensure(64));
 	{ // candidate buffer: sized to the batch (1 per 2 KiB, 1 Mi .. 64 Mi entries); grown on demand by the retry loop below
 		const size_t want = std::min<size_t>(std::max<size_t>(b->bytes / 2048, 1u << 20), 64u << 20);
@@ -841,6 +847,8 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 	A.n_tiles = b->n_tiles;
 	A.cursor = ctx->cursor.p;
 	A.segs = ctx->segs.p;
+	A.occ = ctx->occ.p;
+	A.next_slice = reinterpret_cast<uint32_t *>(ctx->cursor.p + 5);
 	A.scratch = ctx->scratch.p;
 	A.extra_smem = table_bytes;
 	A.spt_shift = spt_shift;
@@ -851,7 +859,7 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 	// general patterns without a candidate filter: no scan kernel -- the VM walk tries the positions itself
 	const bool dense = pat->prog.use_vm && pat->prog.vm_dense;
 	if (dense) {
-		CK(ctx, launch_fill_u32(reinterpret_cast<uint32_t *>(ctx->cursor.p), 8, 0u, ctx->stream));
+		CK(ctx, launch_fill_u32(reinterpret_cast<uint32_t *>(ctx->cursor.p), 12, 0u, ctx->stream));
 		CK(ctx, cudaEventRecord(ctx->ev[1], ctx->stream));
 		S.total_launches += 1;
 	}
@@ -860,7 +868,7 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 		A.cand_cap = (uint32_t)std::min<size_t>(ctx->cand.cap, 0xffffffffu);
 		// a warp reserves candidate slots a chunk at a time; all warps' unused tails together stay below an eighth of the buffer
 		A.chunk = (uint32_t)std::min<size_t>(std::max<size_t>(A.cand_cap / ((size_t)8 * (size_t)grid * (size_t)geom.warps), 32), 1024);
-		CK(ctx, launch_fill_u32(reinterpret_cast<uint32_t *>(ctx->cursor.p), 8, 0u, ctx->stream));
+		CK(ctx, launch_fill_u32(reinterpret_cast<uint32_t *>(ctx->cursor.p), 12, 0u, ctx->stream));
 		CK(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
 		if (hashed) CK(ctx, launch_scan_hash(A, ctx->pat_hash, grid, ctx->stream));
 		else if (pat->prog.kind == ENGINE_FIXED) CK(ctx, launch_scan_fixed(A, ctx->pat_fixed, pat->prog.delta, geom, grid, ctx->stream));
@@ -894,6 +902,7 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 		ResolveArgs R;
 		R.tiles = b->d_tiles;
 		R.segs = ctx->segs.p;
+		R.occ = ctx->occ.p;
 		R.n_segs = n_segs;
 		R.spt_shift = spt_shift;
 		R.tag = ctx->seg_tag;
@@ -1170,12 +1179,12 @@ extern "C" int gscan_tma_probe(gscan_ctx *ctx, gscan_batch *b, int geom, float *
 	const uint32_t n_segs = b->n_tiles << spt_shift;
 	if (ensure_segs(ctx, n_segs) < 0) return -1;
 	CK(ctx, ctx->scratch.ensure((size_t)ctx->num_sms * g.warps * g.slice));
-	CK(ctx, ctx->cursor.ensure(2));
+	CK(ctx, ctx->cursor.ensure(6));
 	if (ctx->cand.cap == 0) CK(ctx, ctx->cand.ensure(1u << 20));
 	ScanArgs A;
 	A.tiles = b->d_tiles; A.n_tiles = b->n_tiles; A.cand = ctx->cand.p; A.cand_cap = (uint32_t)ctx->cand.cap;
-	A.cursor = ctx->cursor.p; A.segs = ctx->segs.p; A.scratch = ctx->scratch.p; A.extra_smem = 0; A.tag = ctx->seg_tag; A.spt_shift = spt_shift; A.chunk = 64;
-	CK(ctx, launch_fill_u32(reinterpret_cast<uint32_t *>(ctx->cursor.p), 8, 0u, ctx->stream));
+	A.cursor = ctx->cursor.p; A.segs = ctx->segs.p; A.occ = ctx->occ.p; A.next_slice = reinterpret_cast<uint32_t *>(ctx->cursor.p + 5); A.scratch = ctx->scratch.p; A.extra_smem = 0; A.tag = ctx->seg_tag; A.spt_shift = spt_shift; A.chunk = 64;
+	CK(ctx, launch_fill_u32(reinterpret_cast<uint32_t *>(ctx->cursor.p), 12, 0u, ctx->stream));
 	CK(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
 	CK(ctx, launch_scan_null(A, geom, (int)std::min<uint32_t>((uint32_t)ctx->num_sms, b->n_tiles), ctx->stream));
 	CK(ctx, cudaEventRecord(ctx->ev[1], ctx->stream));

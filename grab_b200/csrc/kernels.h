@@ -34,6 +34,7 @@ struct FinalRec {
 struct ResolveArgs {
 	const TileDesc *tiles;
 	const SegEntry *segs;
+	uint32_t *occ;        // occupancy bits of segs (ScanArgs::occ); k_gather clears the words it reads
 	uint32_t n_segs;
 	uint32_t spt_shift;   // log2(slices per tile)
 	uint32_t tag;         // generation of the scan that filled segs

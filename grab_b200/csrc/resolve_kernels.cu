@@ -7,7 +7,7 @@
 //      after the first match in FIRST mode (:204-212), skip the rest of the line (<= 511 bytes) in
 //      LINE mode (:194-196)
 //   4. compact the kept records.
-// Traffic: 8 bytes per 2 KiB scanned for the segment table plus O(candidates).
+// Traffic: one occupancy bit per slice scanned, 8 bytes per non-empty slice for the segment table, plus O(candidates).
 #include <cuda_runtime.h>
 #include <cstdint>
 
@@ -54,14 +54,27 @@ __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t *t
 	return r;
 }
 
+// a thread's kPerThread segments [base, base + 8) are 8 bits of one occupancy word: which of them the scan wrote.  Only
+// those entries are read (a sparse pattern over 8 Mi segments reads 1 MiB of bits instead of 64 MiB of entries); a bit
+// left over from an earlier scan is harmless, its entry's generation tag makes it count 0
+static_assert(kPerThread == 8, "one byte of an occupancy word per thread");
+__device__ __forceinline__ uint32_t occ_bits(const uint32_t *occ, uint32_t base, uint32_t n_segs)
+{
+	if (base >= n_segs) return 0u;
+	uint32_t b = (occ[base >> 5] >> (base & 31u)) & 0xffu;
+	if (n_segs - base < 8u) b &= (1u << (n_segs - base)) - 1u;
+	return b;
+}
+
 // ---- 1. segment counts -> block sums ----
-__global__ void k_seg_sums(const SegEntry *segs, uint32_t n_segs, uint32_t tag, uint32_t *blk)
+__global__ void k_seg_sums(const SegEntry *segs, const uint32_t *occ, uint32_t n_segs, uint32_t tag, uint32_t *blk)
 {
 	const uint32_t base = blockIdx.x * kPerBlock + threadIdx.x * kPerThread;
+	const uint32_t bits = occ_bits(occ, base, n_segs);
 	uint32_t s = 0;
 #pragma unroll
 	for (int i = 0; i < kPerThread; i++)
-		if (base + i < n_segs) s += seg_count(segs[base + i], tag);
+		if ((bits >> i) & 1u) s += seg_count(segs[base + i], tag);
 	uint32_t total;
 	block_exclusive_scan(s, &total);
 	if (threadIdx.x == 0) blk[blockIdx.x] = total;
@@ -94,22 +107,26 @@ __global__ void k_scan_blk(uint32_t *blk, uint32_t nb, uint32_t *total_out, uint
 __global__ void k_gather(const ResolveArgs R)
 {
 	const uint32_t base = blockIdx.x * kPerBlock + threadIdx.x * kPerThread;
+	const uint32_t bits = occ_bits(R.occ, base, R.n_segs);
 	uint32_t cnt[kPerThread];
 	uint32_t s = 0;
 #pragma unroll
 	for (int i = 0; i < kPerThread; i++) {
-		cnt[i] = base + i < R.n_segs ? seg_count(R.segs[base + i], R.tag) : 0u;
+		cnt[i] = (bits >> i) & 1u ? seg_count(R.segs[base + i], R.tag) : 0u;
 		s += cnt[i];
 	}
 	uint32_t total;
 	uint32_t p = block_exclusive_scan(s, &total) + R.blk[blockIdx.x];
+	// every thread of the block has read its occupancy byte (the scan above synchronises): clear the word for the next scan
+	if ((base & 31u) == 0 && base < R.n_segs) R.occ[base >> 5] = 0u;
 #pragma unroll
 	for (int i = 0; i < kPerThread; i++) {
 		const uint32_t seg = base + i;
 		if (seg >= R.n_segs) break;
-		const uint32_t tile = seg >> R.spt_shift;
-		const TileDesc td = R.tiles[tile];
-		if (td.off == 0 && (seg & ((1u << R.spt_shift) - 1u)) == 0) R.unit_start[td.unit] = p; // first segment of a unit
+		const bool tile_start = (seg & ((1u << R.spt_shift) - 1u)) == 0;
+		if (!tile_start && !cnt[i]) continue;
+		const TileDesc td = R.tiles[seg >> R.spt_shift];
+		if (tile_start && td.off == 0) R.unit_start[td.unit] = p; // first segment of a unit
 		if (cnt[i]) {
 			const Cand *src = R.cand + R.segs[seg].base;
 			for (uint32_t k = 0; k < cnt[i]; k++) {
@@ -807,7 +824,7 @@ cudaError_t launch_resolve_count(const ResolveArgs &R, cudaStream_t st, uint32_t
 	uint32_t nl = 0;
 	const uint32_t nb_seg = (R.vm_dense || R.vm_ready) ? 0u : (R.n_segs + kPerBlock - 1) / kPerBlock;
 	if (!R.vm_dense && !R.vm_ready) {
-		k_seg_sums<<<nb_seg, kScanBlock, 0, st>>>(R.segs, R.n_segs, R.tag, R.blk); nl++;
+		k_seg_sums<<<nb_seg, kScanBlock, 0, st>>>(R.segs, R.occ, R.n_segs, R.tag, R.blk); nl++;
 		k_scan_blk<<<1, kScanBlock, 0, st>>>(R.blk, nb_seg, R.totals, R.unit_start + R.n_units); nl++;
 		k_gather<<<nb_seg, kScanBlock, 0, st>>>(R); nl++;
 	}

@@ -19,9 +19,10 @@
 // Code size: every instantiation stays under 32 KB of SASS (out-of-line single-copy slow paths), so the
 // rarely executed verification code is still in the SM's instruction cache when a match finally shows up.
 //
-// HBM traffic: every byte once; 8 bytes of segment table per NON-EMPTY slice; candidates
+// HBM traffic: every byte once; 8 bytes of segment table and one occupancy bit per NON-EMPTY slice; candidates
 // only where they exist.
 #include <cuda_runtime.h>
+#include <atomic>
 #include <cstdint>
 #include <cstdlib>
 
@@ -79,20 +80,12 @@ __device__ __forceinline__ uint32_t lop3(uint32_t a, uint32_t b, uint32_t c)
 // L2 eviction policy for the corpus stream: every byte is read exactly once, so its lines are the first to go.
 // Without it the stream (the whole 50 MB L2 turns over every ~15 us) evicts the rarely executed slow-path code and
 // the pattern tables from L2, and a warp that finally hits a match fetches its instructions from DRAM one line at a
-// time.
-#ifndef GS_L2_POLICY
-#define GS_L2_POLICY 0
-#endif
+// time.  On an H100 (80GB HBM3, 400 W limit) evict_first also lifts the literal scan kernel from 2.87 to 2.95 TB/s and
+// the null-consumer ring from 2.95 to 2.98 TB/s against evict_normal (tools/step_budget.py, DESIGN.md section 6).
 __device__ __forceinline__ uint64_t l2_stream_policy()
 {
 	uint64_t p;
-#if GS_L2_POLICY == 1
 	asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-#elif GS_L2_POLICY == 2
-	asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 0.5;" : "=l"(p));
-#else
-	asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
-#endif
 	return p;
 }
 // global -> shared bulk copy executed by the TMA unit; bytes and both addresses multiples of 16
@@ -116,8 +109,10 @@ constexpr uint32_t kHalo = 16;
 struct __align__(16) SlotCtl {
 	uint64_t full;
 	uint64_t src; // global address of tile byte 0
-	uint32_t off, ulen, tile_len, begin, niter, pad;
+	uint32_t off, ulen, tile_len, begin, niter;
+	uint32_t slice; // the slice in the slot; kNoSlice: none, the warp is done once it reaches this slot
 };
+constexpr uint32_t kNoSlice = 0xffffffffu;
 
 // a slot: [16 bytes before the slice, engines with a look-behind only] slice [16 bytes after it]
 size_t scan_smem_bytes(const ScanGeom &g, bool look_behind)
@@ -189,7 +184,12 @@ struct Emitter {
 				for (uint32_t i = lane; i < n; i += 32) A.cand[base + i] = scratch[i];
 				// only non-empty segments are written; the entry carries this scan's generation tag, so stale entries of
 				// earlier scans read as empty and the table never has to be cleared between scans
-				if (lane == 0) A.segs[seg] = SegEntry{base, n | (A.tag << 16)};
+				// the occupancy bit lets the resolve skip the empty segments without reading them; the atomicOr's result
+				// is unused, so it issues as a fire-and-forget reduction and the warp does not wait for it
+				if (lane == 0) {
+					A.segs[seg] = SegEntry{base, n | (A.tag << 16)};
+					atomicOr(&A.occ[seg >> 5], 1u << (seg & 31u));
+				}
 				chunk_base += n;
 				chunk_left -= n;
 			}
@@ -1159,9 +1159,10 @@ struct NullEngine {
 // ------------------------------------------------------------------------------------------
 // the persistent kernel: warp-private TMA rings
 // ------------------------------------------------------------------------------------------
-// Slice s = (tile << spt_shift) + j is the j-th kSlice-byte part of a tile.  Warp g (of all warps of the grid) scans slices g, g + G, g + 2G, ...  Each warp keeps kRing
-// slices in flight: after finishing a slice its lane 0 re-arms the slot's mbarrier and issues the
-// bulk copy for the slice kRing steps ahead.  No producer warp, no "empty" barriers, no __syncthreads.
+// Slice s = (tile << spt_shift) + j is the j-th kSlice-byte part of a tile.  Warp g (of all G warps of the grid) starts with
+// slices g, g + G, ..., g + (kRing - 1) G and then takes runs of slices from a shared counter.  Each warp keeps kRing slices
+// in flight: after finishing a slice its lane 0 re-arms the slot's mbarrier and issues the bulk copy for the warp's next
+// slice.  No producer warp, no "empty" barriers, no __syncthreads.
 template <class G>
 __device__ __forceinline__ void slice_geometry(const TileDesc &d, uint32_t j, uint32_t &begin, uint32_t &niter)
 {
@@ -1204,6 +1205,7 @@ scan_kernel(const __grid_constant__ ScanArgs A, const __grid_constant__ typename
 		uint32_t begin, niter;
 		slice_geometry<G>(d, s & spt_mask, begin, niter);
 		SlotCtl *c = &ctl[slot];
+		c->slice = s;
 		c->src = d.src; c->off = d.off; c->ulen = d.ulen; c->tile_len = d.len; c->begin = begin; c->niter = niter;
 		if (niter == 0) { mbar_arrive(&c->full); return; }
 		const uint32_t rest = (d.ulen - d.off - begin + 15u) & ~15u; // rest of the unit from the slice start, padded to 16
@@ -1229,19 +1231,34 @@ scan_kernel(const __grid_constant__ ScanArgs A, const __grid_constant__ typename
 		for (uint32_t k = 0; k < (uint32_t)G::kRing; k++) {
 			const uint32_t s = first + k * stride;
 			if (s < total) issue(k, s, A.tiles[s >> A.spt_shift]);
+			else ctl[k].slice = kNoSlice;
 		}
 	}
 	__syncwarp();
+	// the first kRing slices of every warp are static (above); every later one comes from a shared counter, kDynRun
+	// consecutive slices per atomicAdd (one counter serves ~500 M atomics/s: one per 4 KiB slice would cap the kernel near
+	// 2 TB/s), so the warps stay together in the stream and an SM that runs ahead takes more slices instead of idling at
+	// the end.  A warp takes its slices in increasing order, so once a slot has no slice, no later slot has one.
+	constexpr uint32_t kDynRun = 4; // a power of two
+	const uint32_t dyn0 = G::kRing * stride;
+	uint32_t run_next = dyn0; // lane 0: the warp's next slice; a new run is taken whenever it reaches a run boundary
 
 	Emitter E;
 	E.scratch = A.scratch + ((size_t)blockIdx.x * G::kWarps + warp) * G::kSlice;
 	E.n = 0;
 	uint32_t slot = 0, phase = 0;
-	for (uint32_t s = first; s < total; s += stride) {
-		// descriptor of the slice that will reuse this slot: fetched now, needed after the scan
-		const uint32_t nxt = s + G::kRing * stride;
+	for (;;) {
+		const uint32_t s = ctl[slot].slice;
+		if (s == kNoSlice) break;
+		// the slice that will reuse this slot and its descriptor: taken now, needed after the scan
+		uint32_t nxt = kNoSlice;
 		TileDesc dn;
-		if (lane == 0 && nxt < total) dn = A.tiles[nxt >> A.spt_shift];
+		if (lane == 0) {
+			if (((run_next - dyn0) & (kDynRun - 1u)) == 0) run_next = dyn0 + atomicAdd(A.next_slice, kDynRun);
+			nxt = run_next < total ? run_next : kNoSlice;
+			run_next++;
+			if (nxt < total) dn = A.tiles[nxt >> A.spt_shift];
+		}
 
 		mbar_wait(&ctl[slot].full, phase);
 		Slice S;
@@ -1256,7 +1273,11 @@ scan_kernel(const __grid_constant__ ScanArgs A, const __grid_constant__ typename
 		Eng::template run<G>(P, S, E, lane);
 		E.flush(A, s, lane);
 		__syncwarp(); // every lane is done reading the slot before it is overwritten
-		if (lane == 0 && nxt < total) issue(slot, nxt, dn);
+		if (lane == 0) {
+			if (nxt < total) issue(slot, nxt, dn);
+			else ctl[slot].slice = kNoSlice;
+		}
+		__syncwarp(); // the slot's slice number is visible to every lane when the warp comes back to it
 		if (++slot == (uint32_t)G::kRing) { slot = 0; phase ^= 1u; }
 	}
 }
@@ -1264,13 +1285,24 @@ scan_kernel(const __grid_constant__ ScanArgs A, const __grid_constant__ typename
 // ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
+constexpr int kMaxDevices = 64;
+
 template <class Eng, class G>
 static cudaError_t launch_g(const ScanArgs &A, const typename Eng::Params &P, int grid, cudaStream_t st)
 {
 	const ScanGeom g{G::kWarps, G::kRing, G::kSlice};
-	const size_t smem = scan_smem_bytes(g, Eng::kLookBehind) + A.extra_smem;
-	cudaError_t e = cudaFuncSetAttribute(scan_kernel<Eng, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	const int smem = (int)(scan_smem_bytes(g, Eng::kLookBehind) + A.extra_smem);
+	// the shared-memory limit is a property of the kernel on a device: raised once per instantiation and device, not per
+	// launch (the largest size asked for so far; the hashed engine's table size varies with the pattern)
+	static std::atomic<int> smem_set[kMaxDevices];
+	int dev = 0;
+	cudaError_t e = cudaGetDevice(&dev);
 	if (e != cudaSuccess) return e;
+	if (dev >= kMaxDevices || smem > smem_set[dev].load(std::memory_order_acquire)) {
+		e = cudaFuncSetAttribute(scan_kernel<Eng, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+		if (e != cudaSuccess) return e;
+		if (dev < kMaxDevices) smem_set[dev].store(smem, std::memory_order_release);
+	}
 	scan_kernel<Eng, G><<<grid, G::kThreads, smem, st>>>(A, P);
 	return cudaGetLastError();
 }
