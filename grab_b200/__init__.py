@@ -18,6 +18,9 @@ UNIT_DEVICE = 1
 UNIT_FD = 2  # ptr carries an open descriptor, the window is [base_off, base_off + len) of it (pread by the engine)
 ENGINE_FIXED, ENGINE_RUN, ENGINE_NONE, ENGINE_VM = 1, 2, 3, 4
 KERNEL_NONE, KERNEL_PAIR, KERNEL_TRIPLE, KERNEL_BALANCED, KERNEL_HASH, KERNEL_RUN = 0, 1, 2, 3, 4, 5
+# Stats.resolve_path (GSCAN_RESOLVE_* of include/gscan.h): how the last scan resolved its candidates
+(RESOLVE_NONE, RESOLVE_WALK, RESOLVE_FLAT, RESOLVE_CHAIN, RESOLVE_VM_ATTEMPTS, RESOLVE_VM_DENSE, RESOLVE_VM_TWO,
+ RESOLVE_VM_DENSE_TWO, RESOLVE_VM_RUN_CHAIN) = range(9)
 
 
 class GscanError(RuntimeError):
@@ -46,7 +49,7 @@ class Stats(ctypes.Structure):
     _fields_ = [("bytes_scanned", ctypes.c_uint64), ("n_candidates", ctypes.c_uint64), ("n_matches", ctypes.c_uint64),
                 ("n_units", ctypes.c_uint32), ("n_tiles", ctypes.c_uint32), ("scan_launches", ctypes.c_uint32),
                 ("total_launches", ctypes.c_uint32), ("scan_kernel_ms", ctypes.c_float), ("resolve_ms", ctypes.c_float),
-                ("h2d_ms", ctypes.c_float), ("total_ms", ctypes.c_float), ("vm_limit_hit", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+                ("h2d_ms", ctypes.c_float), ("total_ms", ctypes.c_float), ("vm_limit_hit", ctypes.c_uint32), ("resolve_path", ctypes.c_uint32)]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}

@@ -109,7 +109,7 @@ struct gscan_ctx {
 	struct ResultBuf { void *p; size_t cap; bool lent; };
 	std::vector<ResultBuf> results;
 	DevBuf<uint32_t> unit_start, unit_out, blk, chain, vm_flag, vm_unit_start;
-	DevBuf<OutRec> vm_ord;
+	DevBuf<OutRec> vm_ord, vm_ord_b;
 	DevBuf<unsigned long long> vm_budget;
 	DevBuf<unsigned long long> cursor; // [0] cursor, [1..4] u32 totals (ResolveArgs::totals), [5] the scan's slice counter
 	DevBuf<uint8_t> pat_tables, hash_tables, vm_tables;
@@ -417,7 +417,7 @@ extern "C" void gscan_close(gscan_ctx *c)
 	cudaSetDevice(c->device);
 	cudaStreamSynchronize(c->stream);
 	c->segs.release(); c->occ.release(); c->cand.release(); c->scratch.release(); c->ord.release(); c->out.release();
-	c->unit_start.release(); c->unit_out.release(); c->blk.release(); c->chain.release(); c->vm_flag.release(); c->vm_unit_start.release(); c->vm_ord.release(); c->vm_budget.release(); c->cursor.release(); c->pat_tables.release(); c->hash_tables.release(); c->vm_tables.release();
+	c->unit_start.release(); c->unit_out.release(); c->blk.release(); c->chain.release(); c->vm_flag.release(); c->vm_unit_start.release(); c->vm_ord.release(); c->vm_ord_b.release(); c->vm_budget.release(); c->cursor.release(); c->pat_tables.release(); c->hash_tables.release(); c->vm_tables.release();
 	c->probe_sum.release(); c->needle.release();
 	c->pool_arena.release(); c->pool_tiles.release(); c->pool_units.release();
 	c->readback.release();
@@ -926,30 +926,44 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 		// unit -- one thread per unit would walk them alone (a 1 GiB window of a log file with a million hits: seconds)
 		R.chain = 0; R.chain_levels = 0; R.chain_cap = 0; R.chain_buf = nullptr;
 		R.vm_par = 0; R.vm_ord = nullptr; R.vm_unit_start = nullptr; R.vm_flag = nullptr; R.vm_budget = nullptr;
+		R.vm_two = 0; R.vm_ord_b = nullptr; R.vm_chain_run = 0; R.vm_limit = R.totals + 2;
+		const bool two = pat->prog.use_vm && !pat->prog.vm_runstart && pat->prog.vm_reach == 1;
 		{
-			// general patterns take the same path when their attempts do not depend on the search start (vm_start_free) and
-			// the candidates come from a leading-sequence filter: one VM attempt per candidate, all at once, then the chain
-			// over the candidates that matched (any mode) -- instead of one thread replaying a huge unit's attempts alone
-			// RUN in LINE mode too: the search resumes behind a line remainder, possibly inside a run (chain_entry)
+			// general patterns take the same path when the candidates come from a leading-sequence filter and an attempt's
+			// outcome depends on the search start at most through the attempt's first byte (vm_reach <= 1; reach 1: two
+			// outcomes per candidate, vm_two), or when they are the run starts of a greedy / possessive leading class repeat
+			// (vm_chain_run): the VM attempts of all candidates at once, then the chain over the ones that matched (any mode)
+			// -- instead of one thread replaying a huge unit's attempts alone.  RUN in LINE mode too: the search resumes behind
+			// a line remainder, possibly inside a run (chain_entry)
 			const bool fixed_ok = !pat->prog.use_vm && ((pat->prog.kind == ENGINE_FIXED && (mode == GSCAN_MODE_ALL || mode == GSCAN_MODE_LINE)) ||
 			                                            (pat->prog.kind == ENGINE_RUN && mode == GSCAN_MODE_LINE));
-			const bool vm_ok = pat->prog.use_vm && !pat->prog.vm_runstart && pat->prog.vm_start_free;
+			const bool run_ok = pat->prog.use_vm && pat->prog.vm_runstart && pat->prog.vm_reach == 0 && pat->prog.vm_lead != VM_Q_LAZY;
+			const bool vm_ok = (pat->prog.use_vm && !pat->prog.vm_runstart && pat->prog.vm_reach <= 1) || run_ok;
 			const bool eligible = !R.flat && !dense && (fixed_ok || vm_ok) && total_cand > 0;
 			bool want = eligible && total_cand >= 65536 && total_cand / std::max<uint64_t>(b->n_units, 1) >= 1024;
 			if (const char *e = getenv("GSCAN_CHAIN")) // tests: force the path on small inputs / switch it off
 				want = eligible && *e == '1';
+			const uint64_t nodes = two ? 2 * total_cand : total_cand;      // vm_two: outcomes A and B of every candidate
+			const uint32_t extra = (two || run_ok) ? 4 : 2;               // marks, ranks (+ the B scan and list / resume points)
 			uint32_t levels = 2; // at least two tables: the second one doubles as the RUN entry positions
-			while ((1ull << levels) < total_cand) levels++;
-			if (want && (uint64_t)(levels + 2) * total_cand * 4 <= (4ull << 30)) {
-				CK(ctx, ctx->chain.ensure((size_t)(levels + 2) * (size_t)total_cand));
-				R.chain = 1; R.chain_levels = levels; R.chain_cap = (uint32_t)total_cand; R.chain_buf = ctx->chain.p;
+			while ((1ull << levels) < nodes) levels++;
+			if (want && (uint64_t)(levels + extra) * nodes * 4 <= (4ull << 30)) {
+				CK(ctx, ctx->chain.ensure((size_t)(levels + extra) * (size_t)nodes));
+				R.chain = 1; R.chain_levels = levels; R.chain_cap = (uint32_t)nodes; R.chain_buf = ctx->chain.p;
 				if (vm_ok) {
-					CK(ctx, ctx->vm_ord.ensure((size_t)total_cand));
-					CK(ctx, ctx->vm_flag.ensure((size_t)total_cand));
+					CK(ctx, ctx->vm_ord.ensure((size_t)nodes));
+					CK(ctx, ctx->vm_flag.ensure((size_t)nodes));
 					CK(ctx, ctx->vm_unit_start.ensure((size_t)b->n_units + 1));
 					CK(ctx, ctx->vm_budget.ensure((size_t)b->n_units));
 					R.vm_budget = ctx->vm_budget.p;
 					R.vm_par = 1; R.vm_ord = ctx->vm_ord.p; R.vm_flag = ctx->vm_flag.p; R.vm_unit_start = ctx->vm_unit_start.p;
+					R.vm_chain_run = run_ok ? 1u : 0u;
+					if (two) {
+						CK(ctx, ctx->vm_ord_b.ensure((size_t)total_cand));
+						CK(ctx, ctx->blk.ensure((size_t)nb_seg + nb_u + (size_t)(nodes / 2048 + 2) + 8));
+						R.blk = ctx->blk.p;
+						R.vm_two = 1; R.vm_ord_b = ctx->vm_ord_b.p;
+					}
 				}
 			}
 		}
@@ -961,7 +975,7 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 		uint32_t nl = 0;
 		uint32_t *h_tot = reinterpret_cast<uint32_t *>((uint8_t *)ctx->readback.p + 16);
 		bool resolved_empty = false;
-		if (dense && pat->prog.vm_start_free) {
+		if (dense && pat->prog.vm_reach <= 1) {
 			// dense general pattern, big units: the attempts of all positions in parallel (k_vm_dense, twice: count / write), then
 			// the chain over the matching positions -- one thread per unit would walk a 1 GiB window for minutes
 			const uint64_t blocks = (uint64_t)b->n_tiles << (b->tile_shift - 6);
@@ -976,6 +990,7 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 				R.blk = ctx->blk.p;
 				R.dense_blocks = (uint32_t)blocks;
 				R.vm_flag = ctx->vm_flag.p; R.vm_budget = ctx->vm_budget.p; R.vm_unit_start = ctx->vm_unit_start.p;
+				R.vm_two = two ? 1u : 0u; // reach 1: both outcomes of every position (the nodes' kinds go beside the chain tables)
 				CK(ctx, launch_vm_dense_count(R, ctx->stream, &nl));
 				S.total_launches += nl;
 				uint32_t *h8 = reinterpret_cast<uint32_t *>((uint8_t *)ctx->readback.p + 32);
@@ -987,21 +1002,28 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 				if (hits == 0) {
 					h_tot[0] = 0; h_tot[1] = 0; h_tot[2] = h8[2];
 					resolved_empty = true;
-				} else if ((uint64_t)(levels + 2) * hits * 4 <= (4ull << 30)) {
+				} else if ((uint64_t)(levels + (two ? 4 : 2)) * hits * 4 <= (4ull << 30)) {
 					CK(ctx, ctx->vm_ord.ensure((size_t)hits));
-					CK(ctx, ctx->chain.ensure((size_t)(levels + 2) * (size_t)hits));
+					CK(ctx, ctx->chain.ensure((size_t)(levels + (two ? 4 : 2)) * (size_t)hits));
 					CK(ctx, ctx->blk.ensure((size_t)(blocks / 2048 + 2) + nb_u + (size_t)(hits / 2048 + 2) + 16));
 					R.blk = ctx->blk.p;
 					R.vm_ord = ctx->vm_ord.p;
+					R.chain = 1; R.chain_levels = levels; R.chain_cap = (uint32_t)hits; R.chain_buf = ctx->chain.p; // vm_two: the write pass fills chain_bscan
 					CK(ctx, launch_vm_dense_write(R, ctx->stream, &nl));
 					S.total_launches += nl;
 					R.vm_par = 1; R.vm_ready = 1; R.vm_dense = 0;
-					R.chain = 1; R.chain_levels = levels; R.chain_cap = (uint32_t)hits; R.chain_buf = ctx->chain.p;
 					R.total_cand = (uint32_t)hits;
-					S.n_candidates = hits; // positions where an attempt matched
-				} // else: more matching positions than the chain tables may hold -- the per-unit walk below serves the batch
+					S.n_candidates = hits; // matching outcomes (vm_two: A and B counted apart)
+				} else {
+					R.vm_two = 0; // more matching positions than the chain tables may hold -- the per-unit walk below serves the batch
+				}
 			}
 		}
+		S.resolve_path = resolved_empty ? (R.vm_two ? GSCAN_RESOLVE_VM_DENSE_TWO : GSCAN_RESOLVE_VM_DENSE)
+		               : R.vm_chain_run ? GSCAN_RESOLVE_VM_RUN_CHAIN
+		               : R.vm_par ? (R.vm_ready ? (R.vm_two ? GSCAN_RESOLVE_VM_DENSE_TWO : GSCAN_RESOLVE_VM_DENSE)
+		                                        : (R.vm_two ? GSCAN_RESOLVE_VM_TWO : GSCAN_RESOLVE_VM_ATTEMPTS))
+		               : R.chain ? GSCAN_RESOLVE_CHAIN : R.flat ? GSCAN_RESOLVE_FLAT : GSCAN_RESOLVE_WALK;
 		if (!resolved_empty) {
 			CK(ctx, launch_resolve_count(R, ctx->stream, &nl));
 			S.total_launches += nl;

@@ -78,7 +78,20 @@ struct ResolveArgs {
 	uint32_t vm_ready;        // vm_ord / vm_unit_start are filled already: no segments, no gather, no k_vm_attempts
 	uint32_t dense_blocks;    // 64-position blocks of the batch = n_tiles << (dense_tile_shift - 6)
 	uint32_t dense_tile_shift;
-	uint32_t vm_dense;    // general pattern without a candidate filter: no candidate list, the walk offers every position whose byte
+	// reach-1 programs on the chain paths (vm_two, with vm_par; Program::vm_reach == 1: only the attempt whose subject begins at
+	// the candidate itself differs from "any earlier start").  Every candidate p gets two outcomes, A(p): subject begins at p,
+	// and B(p): subject begins before p (p >= 1).  The matching ones form one node list in (unit, pos, A before B) order; a
+	// search that resumes at s continues at node (s, A) if A(s) matched, else at the first B node behind s.  Which nodes are
+	// B is kept beside the chain tables (chain_bscan: exclusive count of B nodes, chain_blist: their indices, totals[5] of
+	// them), never in OutRec.  vm_ord_b: [total_cand] the B outcomes of k_vm_attempts, before compaction.
+	uint32_t vm_two;
+	OutRec *vm_ord_b;
+	// class-repeat-led programs on the chain path (vm_chain_run, with vm_par; vm_runstart, reach 0, greedy or possessive lead):
+	// a search that resumes inside a run tries one attempt there; if it matches it ends where the run start's own match ends
+	// (chain_stop: where each node's search resumes, for chain_entry)
+	uint32_t vm_chain_run;
+	uint32_t *vm_limit;   // vm_chain_run: the VM limit flag (totals[2]; the chain kernels see totals + 4)
+	uint32_t vm_dense;   // general pattern without a candidate filter: no candidate list, the walk offers every position whose byte
 	                      // is in `bitmap` (the first-byte set) to the VM
 	uint32_t flat;        // ALL mode, RUN or a FIXED pattern whose matches can never overlap, no VM: every candidate of a unit is a
 	                      // match, except that the loop guard (grab.cc:175, Q1) can drop the unit's LAST one -- no replay needed, the

@@ -859,6 +859,57 @@ struct VmGen {
 	}
 };
 
+// Reach of a VM program (Program::vm_reach): an attempt at p reads the subject's beginning s only where a back-looking
+// construct runs close to it -- an assertion that tests sp == 0 or the byte before sp (^ \A (?m)^ \b \B), or a look-behind
+// of b bytes, which fails / holds at once when fewer than b bytes precede sp.  Run at offset o >= m from p, such a construct
+// sees the same as from any earlier start once s <= p + m - 1 (assertions) or s <= p + m - b (look-behinds).  `m` is the
+// least offset at which the node can begin (negative inside a look-behind body); returns the least offset behind it.
+int64_t reach_walk(const Node *n, int64_t m, int64_t &reach)
+{
+	switch (n->kind) {
+	case Node::EMPTY: return m;
+	case Node::SET: return m + 1;
+	case Node::ASSERT:
+		if (n->akind == VM_A_BOL || n->akind == VM_A_SOS || n->akind == VM_A_MBOL || n->akind == VM_A_WORDB || n->akind == VM_A_NWORDB)
+			reach = std::max<int64_t>(reach, 1 - m);
+		return m;
+	case Node::GROUP: case Node::ATOMIC: return reach_walk(n->kids[0].get(), m, reach);
+	case Node::LOOK: {
+		if (n->ahead) { reach_walk(n->kids[0].get(), m, reach); return m; }
+		const Node *body = peel_noncapturing(n->kids[0].get()); // one fixed length per top-level branch, as VmGen emits it
+		std::vector<const Node *> branches;
+		if (body->kind == Node::ALT) for (auto &k : body->kids) branches.push_back(k.get());
+		else branches.push_back(body);
+		for (const Node *br : branches) {
+			uint64_t len = 0;
+			fixed_length(br, len);
+			reach = std::max<int64_t>(reach, (int64_t)len - m);
+			reach_walk(br, m - (int64_t)len, reach);
+		}
+		return m;
+	}
+	case Node::CAT:
+		for (auto &k : n->kids) m = reach_walk(k.get(), m, reach);
+		return m;
+	case Node::ALT: {
+		int64_t lo = INT64_MAX;
+		for (auto &k : n->kids) lo = std::min(lo, reach_walk(k.get(), m, reach));
+		return lo;
+	}
+	case Node::REP: // later iterations begin at or behind the first one: the first bounds them all
+		reach_walk(n->kids[0].get(), m, reach);
+		return m + (int64_t)n->rmin * (int64_t)min_length(n->kids[0].get());
+	}
+	return m;
+}
+
+int vm_reach(const Node *root)
+{
+	int64_t reach = 0;
+	reach_walk(root, 0, reach);
+	return (int)std::min<int64_t>(reach, 1 << 20);
+}
+
 // byte-class sequences (length <= L) every match of `n` starts with; `done`: the node is consumed exactly by
 // the sequence, so what follows the node may extend it
 struct Pref { Sequence seq; bool done; };
@@ -1093,6 +1144,8 @@ bool compile_pattern(const char *pat, size_t len, uint32_t flags, Program &out, 
 		g.gen(root.get());
 		g.emit(VM_MATCH, 0, 0, 0, 0);
 		if (g.failed) { err = g.why; return false; }
+		out.vm_reach = vm_reach(root.get());
+		out.vm_start_free = out.vm_reach == 0;
 		// a pattern that begins with a greedy/lazy/possessive byte-class repeat C{n,}: if an attempt succeeds anywhere
 		// inside a run of C it also succeeds at the run's first byte (C{n,} simply takes the bytes in between), so
 		// PCRE's leftmost match starts at a run start -- or at the search start itself when that lies inside a run.
@@ -1118,6 +1171,7 @@ bool compile_pattern(const char *pat, size_t len, uint32_t flags, Program &out, 
 						out.maxlen = -1;
 						out.use_vm = true;
 						out.vm_runstart = true;
+						out.vm_lead = lead->lazy ? VM_Q_LAZY : lead->possessive ? VM_Q_POSSESSIVE : VM_Q_GREEDY;
 						out.vm_code = g.code;
 						for (auto &s : g.sets) for (int i = 0; i < 8; i++) out.vm_sets.push_back(s.w[i]);
 						return true;
@@ -1128,12 +1182,6 @@ bool compile_pattern(const char *pat, size_t len, uint32_t flags, Program &out, 
 		std::vector<Pref> pf;
 		out.use_vm = true;
 		out.vm_code = g.code;
-		out.vm_start_free = true;
-		for (size_t i = 0; i + 2 < out.vm_code.size(); i += 3) {
-			const uint32_t op = out.vm_code[i] & 0xffu, kind = (out.vm_code[i] >> 8) & 0xffu;
-			if (op == VM_ASSERT && (kind == VM_A_BOL || kind == VM_A_SOS || kind == VM_A_WORDB || kind == VM_A_NWORDB || kind == VM_A_MBOL)) out.vm_start_free = false;
-			if (op == VM_LOOK && (kind == VM_LK_BEHIND || kind == VM_LK_BEHIND_NEG)) out.vm_start_free = false;
-		}
 		for (auto &s : g.sets) for (int i = 0; i < 8; i++) out.vm_sets.push_back(s.w[i]);
 		bool dense = !prefixes(root.get(), 4, pf) || pf.empty();
 		seqs.clear();

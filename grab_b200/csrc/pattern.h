@@ -103,9 +103,12 @@ struct Program {
 	bool vm_dense = false;         // no useful candidate filter (the match can begin with (almost) any byte): the VM walk tries every
 	                               // position whose byte is in first_set itself, no scan kernel runs -- PCRE does the same on the CPU
 	ByteSet first_set;             // vm_dense: bytes a match can start with
-	bool vm_start_free = false;    // no instruction looks at or before the attempt's first byte (^ \A \b \B (?m)^, look-behinds): an
-	                               // anchored attempt at a position gives the same result wherever the subject begins, so the
-	                               // attempts of a unit's candidates can run in parallel (resolve: ResolveArgs::vm_par)
+	int vm_reach = 0;              // sound upper bound L: an attempt at p has the same outcome for every subject beginning s <= p - L
+	                               // (only ^ \A \b \B (?m)^ and look-behinds near the attempt's first byte look at s; 1: the
+	                               // attempt at s itself differs from "any earlier start", resolve: ResolveArgs::vm_two)
+	bool vm_start_free = false;    // vm_reach == 0: an anchored attempt at a position gives the same result wherever the subject
+	                               // begins, so the attempts of a unit's candidates can run in parallel (resolve: ResolveArgs::vm_par)
+	int vm_lead = 0;               // vm_runstart: VM_Q_* of the leading repeat (after (?U))
 	std::vector<uint32_t> vm_code; // 3 words per instruction
 	std::vector<uint32_t> vm_sets; // 8 words per byte class
 

@@ -420,6 +420,31 @@ constexpr uint32_t kChainEnd = 0xffffffffu;
 __device__ __forceinline__ uint32_t *chain_level(const ResolveArgs &R, uint32_t k) { return R.chain_buf + (size_t)k * R.chain_cap; }
 __device__ __forceinline__ uint32_t *chain_mark(const ResolveArgs &R) { return R.chain_buf + (size_t)R.chain_levels * R.chain_cap; }
 __device__ __forceinline__ uint32_t *chain_rank(const ResolveArgs &R) { return R.chain_buf + (size_t)(R.chain_levels + 1) * R.chain_cap; }
+// vm_two: is-B flag of every node, then (in place) its exclusive scan; the B nodes' indices in order.  vm_chain_run: where each
+// node's search resumes, and the outcome of the attempt there (k_vm_resume)
+__device__ __forceinline__ uint32_t *chain_bscan(const ResolveArgs &R) { return R.chain_buf + (size_t)(R.chain_levels + 2) * R.chain_cap; }
+__device__ __forceinline__ uint32_t *chain_blist(const ResolveArgs &R) { return R.chain_buf + (size_t)(R.chain_levels + 3) * R.chain_cap; }
+__device__ __forceinline__ uint32_t *chain_stop(const ResolveArgs &R) { return chain_bscan(R); }
+__device__ __forceinline__ uint32_t *chain_resume(const ResolveArgs &R) { return chain_blist(R); }
+
+// vm_two, chain view (totals[0]: nodes, totals[1]: B nodes): node j is a B node when the exclusive count steps behind it
+__device__ __forceinline__ bool two_is_b(const ResolveArgs &R, uint32_t j)
+{
+	const uint32_t *bs = chain_bscan(R);
+	return (j + 1 < R.totals[0] ? bs[j + 1] : R.totals[1]) != bs[j];
+}
+// vm_two: where a search that resumes at `s` goes on -- lo: the unit's first node at or after s, uend: the unit's end.  Node
+// (s, A) if A(s) matched; else the first B node behind s (B(s) itself is never taken: the subject began AT s)
+__device__ __forceinline__ uint32_t two_next(const ResolveArgs &R, uint32_t lo, uint32_t uend, uint64_t s)
+{
+	if (lo < uend && R.ord[lo].pos == s && !two_is_b(R, lo)) return lo;
+	while (lo < uend && R.ord[lo].pos == s) lo++; // at most the two nodes of s
+	if (lo >= uend) return kChainEnd;
+	const uint32_t j = chain_bscan(R)[lo];
+	if (j >= R.totals[1]) return kChainEnd;
+	const uint32_t b = chain_blist(R)[j];
+	return b < uend ? b : kChainEnd;
+}
 
 // next(i): where the loop resumes behind match i (grab.cc:209; LINE mode: behind the line remainder, <= 511 bytes,
 // grab.cc:194-196), the guard of the next iteration (grab.cc:175), then the first candidate of the unit at or after it
@@ -446,23 +471,27 @@ __global__ void k_chain_next(const ResolveArgs R)
 	}
 	if (run) R.ord[i].pad = (uint32_t)stop; // where the search resumes behind this match (k_chain_entry)
 	uint32_t nx = kChainEnd;
+	if (R.vm_chain_run && chain_resume(R)[i] == 2u) stop = ulen; // the attempt where the search resumes ran into the VM limit
 	if (stop + R.minlen < ulen) {
 		// RUN: the search may resume INSIDE a run (behind a line remainder); if what is left of that run is long enough the
 		// leftmost match is at `stop` itself -- it ends where the run's own candidate ends, so the chain goes on from that
-		// candidate and only the reported start differs (chain_entry)
+		// candidate and only the reported start differs (chain_entry).  vm_chain_run: k_vm_resume ran the attempt there
 		bool inside = false;
 		if (run && stop > 0 && in_class(R, data[stop - 1]) && in_class(R, data[stop])) {
 			uint64_t e = stop;
 			while (e < ulen && in_class(R, data[e])) e++;
 			inside = e - stop >= R.run_min;
 		}
-		uint32_t lo = i + 1, hi = R.unit_start[c.unit + 1]; // candidates are ordered by position inside the unit
+		if (R.vm_chain_run) inside = chain_resume(R)[i] == 1u;
+		const uint32_t uend = R.unit_start[c.unit + 1];
+		uint32_t lo = i + 1, hi = uend; // candidates are ordered by position inside the unit
 		while (lo < hi) {
 			const uint32_t mid = lo + ((hi - lo) >> 1);
 			if (R.ord[mid].pos < stop) lo = mid + 1; else hi = mid;
 		}
-		if (inside) nx = lo - 1; // the run that holds `stop`: the last one that starts before it (behind i's own run)
-		else if (lo < R.unit_start[c.unit + 1]) nx = lo;
+		if (R.vm_two) nx = two_next(R, lo, uend, stop);
+		else if (inside) nx = lo > i + 1 ? lo - 1 : kChainEnd; // the run that holds `stop`: the last one that starts before it (behind i's own run)
+		else if (lo < uend) nx = lo;
 	}
 	chain_level(R, 0)[i] = nx;
 }
@@ -482,8 +511,10 @@ __global__ void k_chain_heads(const ResolveArgs R)
 {
 	const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
 	if (u >= R.n_units) return;
-	const uint32_t first = R.unit_start[u];
-	if (first != R.unit_start[u + 1] && R.minlen < (uint64_t)R.units[u].len) chain_mark(R)[first] = 1u;
+	const uint32_t first = R.unit_start[u], end = R.unit_start[u + 1];
+	if (first == end || !(R.minlen < (uint64_t)R.units[u].len)) return;
+	const uint32_t h = R.vm_two ? two_next(R, first, end, 0u) : first; // vm_two: the first search begins at 0
+	if (h != kChainEnd) chain_mark(R)[h] = 1u;
 }
 
 // descending levels: after level k every chain member whose distance from the head has no bit below k is marked.
@@ -513,7 +544,7 @@ __global__ void k_chain_entry(const ResolveArgs R)
 	if (!chain_mark(R)[i]) return;
 	const uint32_t nx = chain_level(R, 0)[i];
 	if (nx == kChainEnd) return;
-	const uint32_t stop = R.ord[i].pad;
+	const uint32_t stop = R.vm_chain_run ? chain_stop(R)[i] : R.ord[i].pad;
 	if (stop > R.ord[nx].pos) chain_entry(R)[nx] = stop; // one marked predecessor per chain member: no two writers
 }
 
@@ -545,7 +576,7 @@ __global__ void k_chain_write(const ResolveArgs R)
 	const OutRec c = R.ord[i];
 	const DevUnit du = R.units[c.unit];
 	const uint32_t k = chain_rank(R)[i] - chain_rank(R)[R.unit_start[c.unit]];
-	const uint32_t from = R.engine == GSCAN_ENGINE_RUN ? chain_entry(R)[i] : c.pos;
+	const uint32_t from = (R.engine == GSCAN_ENGINE_RUN || R.vm_chain_run) ? chain_entry(R)[i] : c.pos;
 	FinalRec r;
 	r.start = du.base_off + from;
 	r.file_id = du.file_id;
@@ -571,23 +602,47 @@ __global__ void __launch_bounds__(64, 4) k_vm_attempts(const ResolveArgs R)
 	if (rc < 0) { atomicOr(R.totals + 2, 1u); rc = 3; }
 	R.ord[i].len = e;             // the subject began at the candidate: the end offset is the match length
 	R.ord[i].pad = (uint32_t)rc;  // 0: no match here, 1: match, 2: match with a capturing group set (Q2), 3: VM limit
-	R.vm_flag[i] = rc != 0 ? 1u : 0u;
+	if (!R.vm_two) { R.vm_flag[i] = rc != 0 ? 1u : 0u; return; }
+	// vm_two: B(p), the subject begins one byte before the candidate -- what every earlier search start sees (reach 1)
+	OutRec b;
+	b.unit = c.unit; b.pos = c.pos; b.len = 0; b.pad = 0;
+	if (c.pos >= 1u) {
+		budget.new_search();
+		uint32_t eb = 0;
+		int rb = vm_exec(R, data + c.pos - 1u, du.len - c.pos + 1u, 1u, &eb, budget);
+		budget.give_back();
+		if (rb < 0) { atomicOr(R.totals + 2, 1u); rb = 3; }
+		if (rb == 1 || rb == 2) b.len = eb - 1u;
+		b.pad = (uint32_t)rb;
+	}
+	R.vm_ord_b[i] = b;
+	R.vm_flag[2 * i] = rc != 0 ? 1u : 0u;
+	R.vm_flag[2 * i + 1] = b.pad != 0 ? 1u : 0u;
 }
 
+// vm_two / vm_chain_run: the budget covers two attempts per position (A and B; a run start and a search resuming inside its
+// run), twice what the serial walk gets -- it makes one attempt per position and search
 __global__ void k_vm_budget_init(const ResolveArgs R)
 {
 	const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
 	if (u >= R.n_units) return;
-	R.vm_budget[u] = VmBudget::unit_total(R.units[u].len);
+	R.vm_budget[u] = VmBudget::unit_total(R.units[u].len) << ((R.vm_two || R.vm_chain_run) ? 1 : 0);
 }
 
-// vm_flag holds its own exclusive scan by now: the candidates that matched, in order
+// vm_flag holds its own exclusive scan by now: the candidates that matched, in order (vm_two: A then B of every candidate,
+// and the node's kind into chain_bscan)
 __global__ void k_vm_compact(const ResolveArgs R)
 {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= R.totals[0]) return;
 	const OutRec c = R.ord[i];
-	if (c.pad) R.vm_ord[R.vm_flag[i]] = c;
+	if (!R.vm_two) {
+		if (c.pad) R.vm_ord[R.vm_flag[i]] = c;
+		return;
+	}
+	const OutRec b = R.vm_ord_b[i];
+	if (c.pad) { R.vm_ord[R.vm_flag[2 * i]] = c; chain_bscan(R)[R.vm_flag[2 * i]] = 0u; }
+	if (b.pad) { R.vm_ord[R.vm_flag[2 * i + 1]] = b; chain_bscan(R)[R.vm_flag[2 * i + 1]] = 1u; }
 }
 
 // first matching candidate of every unit (R.totals[4]: how many matched in all)
@@ -596,7 +651,46 @@ __global__ void k_vm_unit_starts(const ResolveArgs R)
 	const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
 	if (u > R.n_units) return;
 	const uint32_t s = R.unit_start[u];
-	R.vm_unit_start[u] = s < R.totals[0] ? R.vm_flag[s] : R.totals[4];
+	R.vm_unit_start[u] = s < R.totals[0] ? R.vm_flag[R.vm_two ? 2 * s : s] : R.totals[4];
+}
+
+// vm_two, chain view, chain_bscan scanned: the index of every B node at its rank among them
+__global__ void k_two_blist(const ResolveArgs R)
+{
+	const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+	if (j >= R.totals[0]) return;
+	if (two_is_b(R, j)) chain_blist(R)[chain_bscan(R)[j]] = j;
+}
+
+// vm_chain_run, chain view: where the search resumes behind node i, and -- when that lies inside a run of the leading class
+// (the test of k_walk_vm) -- the attempt there: 1 match (it ends where the run start's own match ends: a greedy or possessive
+// C{n,} from inside the run tries a subset of the run start's split points, in the same order), 0 none, 2 VM limit.  Own
+// kernel: the VM's thread-local stack stays out of the chain kernels
+__global__ void __launch_bounds__(64, 4) k_vm_resume(const ResolveArgs R)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= R.totals[0]) return;
+	const OutRec c = R.ord[i];
+	const DevUnit du = R.units[c.unit];
+	const uint64_t ulen = du.len;
+	const uint8_t *data = reinterpret_cast<const uint8_t *>(du.ptr);
+	uint64_t stop = (uint64_t)c.pos + c.len;
+	if (R.mode == GSCAN_MODE_LINE) {
+		uint32_t a = 0;
+		while (stop + a < ulen && a < 511 && data[stop + a] != '\n') a++;
+		stop += a;
+	}
+	chain_stop(R)[i] = (uint32_t)stop;
+	uint32_t res = 0;
+	if (c.pad < 2u && stop + R.minlen < ulen && stop > 0 && in_class(R, data[stop - 1]) && in_class(R, data[stop])) {
+		VmBudget budget(ulen, R.vm_budget + c.unit);
+		uint32_t e = 0;
+		const int rc = vm_exec(R, data + stop, (uint32_t)(ulen - stop), 0u, &e, budget);
+		budget.give_back();
+		if (rc < 0) { atomicOr(R.vm_limit, 1u); res = 2; }
+		else res = rc != 0 ? 1u : 0u;
+	}
+	chain_resume(R)[i] = res;
 }
 
 // ---- dense general patterns on the chain path (ResolveArgs::vm_ready) ----
@@ -624,24 +718,34 @@ __global__ void __launch_bounds__(64, 4) k_vm_dense(const ResolveArgs R)
 		const uint32_t ulen = du.len;
 		const uint32_t hi = lo + (1u << kDenseShift) < tile_end ? lo + (1u << kDenseShift) : tile_end;
 		VmBudget budget(ulen, R.vm_budget + td.unit);
-		for (uint32_t pos = lo; pos < hi; pos++) {
+		// vm_two: both outcomes of every position, A (subject begins at pos) before B (subject begins at pos - 1); the write
+		// pass records each node's kind in chain_bscan
+		const uint32_t kinds = R.vm_two ? 2u : 1u;
+		for (uint32_t pos = lo; pos < hi && !(WRITE && n == cnt); pos++) {
 			if ((uint64_t)pos + R.minlen > ulen) break;                                 // an attempt with fewer bytes left cannot succeed
 			if (!in_class(R, data[pos])) continue;
-			uint32_t e = 0;
-			int rc = vm_exec(R, data + pos, ulen - pos, 0u, &e, budget);
-			budget.new_search();
-			if (rc < 0) { atomicOr(R.totals + 2, 1u); rc = 3; }
-			if (rc == 0) continue;
-			if (WRITE) {
-				if (n == cnt) break;
-				OutRec r;
-				r.unit = td.unit; r.pos = pos; r.len = e; r.pad = (uint32_t)rc;
-				o[n] = r;
+			for (uint32_t k = 0; k < kinds; k++) {
+				if (k == 1u && pos == 0u) break;
+				uint32_t e = 0;
+				int rc = vm_exec(R, data + pos - k, ulen - pos + k, k, &e, budget);
+				budget.new_search();
+				if (rc < 0) { atomicOr(R.totals + 2, 1u); rc = 3; }
+				if (rc == 0) continue;
+				if (WRITE) {
+					if (n == cnt) break;
+					OutRec r;
+					r.unit = td.unit; r.pos = pos; r.len = rc == 3 ? 0u : e - k; r.pad = (uint32_t)rc;
+					o[n] = r;
+					if (R.vm_two) chain_bscan(R)[R.vm_flag[b] + n] = k;
+				}
+				n++;
 			}
-			n++;
 		}
 		budget.give_back();
-		if (WRITE) for (; n < cnt; n++) { OutRec r; r.unit = td.unit; r.pos = hi - 1u; r.len = 0; r.pad = 3u; o[n] = r; }
+		if (WRITE) for (; n < cnt; n++) {
+			OutRec r; r.unit = td.unit; r.pos = hi - 1u; r.len = 0; r.pad = 3u; o[n] = r;
+			if (R.vm_two) chain_bscan(R)[R.vm_flag[b] + n] = 1u; // keeps the (pos, A before B) order
+		}
 	}
 	if (!WRITE) R.vm_flag[b] = n;
 }
@@ -834,8 +938,10 @@ cudaError_t launch_resolve_count(const ResolveArgs &R, cudaStream_t st, uint32_t
 		// grids cover the reserved candidate slots; the kernels stop at the exact count (totals[0], on the device by now)
 		const uint32_t nb_c = (R.chain_cap + 255) / 256, nb_cs = (R.chain_cap + kPerBlock - 1) / kPerBlock;
 		uint32_t *blk3 = blk2 + nb_u + 1;
+		uint32_t *bscan = chain_mark_host(R) + 2u * (size_t)R.chain_cap; // vm_two: chain_bscan
 		if (R.vm_par && !R.vm_ready) {
-			k_fill_zero<<<nb_c, 256, 0, st>>>(R.vm_flag, R.chain_cap); nl++;
+			k_fill_zero<<<nb_c, 256, 0, st>>>(R.vm_flag, R.chain_cap); nl++; // vm_two: chain_cap is two slots per candidate
+			if (R.vm_two) { k_fill_zero<<<nb_c, 256, 0, st>>>(bscan, R.chain_cap); nl++; }
 			k_vm_budget_init<<<(R.n_units + 255) / 256, 256, 0, st>>>(R); nl++;
 			k_vm_attempts<<<(R.chain_cap + 63) / 64, 64, 0, st>>>(R); nl++;
 			k_u32_sums<<<nb_cs, kScanBlock, 0, st>>>(R.vm_flag, R.chain_cap, blk3); nl++;
@@ -845,18 +951,25 @@ cudaError_t launch_resolve_count(const ResolveArgs &R, cudaStream_t st, uint32_t
 			k_vm_unit_starts<<<(R.n_units + 1 + 255) / 256, 256, 0, st>>>(R); nl++;
 		}
 		const ResolveArgs C = chain_view(R);
+		if (R.vm_two) { // which nodes are B: exclusive count (total: totals[5]) and the list of their indices
+			k_u32_sums<<<nb_cs, kScanBlock, 0, st>>>(bscan, C.chain_cap, blk3); nl++;
+			k_scan_blk<<<1, kScanBlock, 0, st>>>(blk3, nb_cs, R.totals + 5, nullptr); nl++;
+			k_u32_exclusive<<<nb_cs, kScanBlock, 0, st>>>(bscan, C.chain_cap, blk3); nl++;
+			k_two_blist<<<nb_c, 256, 0, st>>>(C); nl++;
+		}
 		const bool follow = R.mode != GSCAN_MODE_FIRST; // FIRST: the head of every unit's chain is all there is
 		k_fill_zero<<<nb_c, 256, 0, st>>>(chain_mark_host(C), 2u * C.chain_cap); nl++; // marks and ranks
 		if (follow) {
+			if (R.vm_chain_run) { k_vm_resume<<<(C.chain_cap + 63) / 64, 64, 0, st>>>(C); nl++; }
 			k_chain_next<<<nb_c, 256, 0, st>>>(C); nl++;
 			for (uint32_t k = 1; k < C.chain_levels; k++) { k_chain_double<<<nb_c, 256, 0, st>>>(C, k); nl++; }
 		}
 		k_chain_heads<<<(C.n_units + 255) / 256, 256, 0, st>>>(C); nl++;
 		if (follow) for (uint32_t k = C.chain_levels; k-- > 0;) { k_chain_spread<<<nb_c, 256, 0, st>>>(C, k); nl++; }
 		if (R.vm_par) { k_chain_unmark<<<nb_c, 256, 0, st>>>(C); nl++; }
-		if (R.engine == GSCAN_ENGINE_RUN) {
+		if (R.engine == GSCAN_ENGINE_RUN || R.vm_chain_run) {
 			k_chain_entry_init<<<nb_c, 256, 0, st>>>(C); nl++;
-			k_chain_entry<<<nb_c, 256, 0, st>>>(C); nl++;
+			if (follow) { k_chain_entry<<<nb_c, 256, 0, st>>>(C); nl++; }
 		}
 		cudaMemcpyAsync(chain_mark_host(C) + C.chain_cap, chain_mark_host(C), (size_t)C.chain_cap * 4, cudaMemcpyDeviceToDevice, st);
 		k_u32_sums<<<nb_cs, kScanBlock, 0, st>>>(chain_mark_host(C) + C.chain_cap, C.chain_cap, blk3); nl++;
@@ -899,7 +1012,9 @@ cudaError_t launch_vm_dense_write(const ResolveArgs &R, cudaStream_t st, uint32_
 cudaError_t launch_resolve_write(const ResolveArgs &R, cudaStream_t st, uint32_t *launches)
 {
 	if (R.chain) {
-		k_chain_write<<<(R.total_cand + 255) / 256, 256, 0, st>>>(chain_view(R));
+		ResolveArgs C = chain_view(R);
+		if (R.vm_two) C.total_cand = R.chain_cap; // two node slots per candidate; the slots behind the nodes are unmarked
+		k_chain_write<<<(C.total_cand + 255) / 256, 256, 0, st>>>(C);
 		if (launches) *launches = 1;
 		return cudaGetLastError();
 	}

@@ -105,8 +105,20 @@ typedef struct gscan_stats {
 	uint32_t vm_limit_hit;   /* != 0: on at least one unit the device VM ran out of backtracking stack (2048 frames) or steps;
 	                            that unit's loop stopped there, as the reference's does when pcre_exec returns an error
 	                            (grab.cc:179, quirk Q5) -- the matches before it and all other units are complete */
-	uint32_t reserved;
+	uint32_t resolve_path;   /* GSCAN_RESOLVE_* below: how the last call turned candidates into the reference loop's matches */
 } gscan_stats;
+
+#define GSCAN_RESOLVE_NONE 0         /* nothing to resolve (no candidates) */
+#define GSCAN_RESOLVE_WALK 1         /* one GPU thread replays each unit's loop (slow on a single huge window with many candidates) */
+#define GSCAN_RESOLVE_FLAT 2         /* ALL mode, matches that cannot overlap: one thread per candidate */
+#define GSCAN_RESOLVE_CHAIN 3        /* FIXED / RUN: pointer doubling over the candidates */
+#define GSCAN_RESOLVE_VM_ATTEMPTS 4  /* general pattern, start-free: one VM attempt per candidate, then the chain */
+#define GSCAN_RESOLVE_VM_DENSE 5     /* general pattern without a candidate filter, start-free: attempts at all positions, then the chain */
+#define GSCAN_RESOLVE_VM_TWO 6       /* as VM_ATTEMPTS for patterns that look one byte behind the search start (^ \b (?<=x) ...):
+                                        two attempts per candidate */
+#define GSCAN_RESOLVE_VM_DENSE_TWO 7 /* as VM_DENSE, two attempts per position */
+#define GSCAN_RESOLVE_VM_RUN_CHAIN 8 /* general pattern led by a greedy / possessive class repeat (\w+@...): attempts at the run
+                                        starts, one more where a search resumes inside a run, then the chain */
 
 /* ---- pattern: replaces FileGrep::prepare (grab.cc:101-123) ----------------------------- */
 
