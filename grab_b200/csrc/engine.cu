@@ -23,6 +23,7 @@
 #include "../../include/gscan.h"
 #include "device_types.h"
 #include "kernels.h"
+#include "resolve_plan.h"
 #include "pattern.h"
 
 using namespace gscan;
@@ -893,13 +894,21 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 	size_t n = 0;
 	gscan_match *m = nullptr;
 	static_assert(sizeof(FinalRec) == sizeof(gscan_match), "device records are gscan_match");
-	if (total_cand || dense) {
-		const uint32_t nb_seg = (n_segs + 2047) / 2048, nb_u = (uint32_t)((b->n_units + 2047) / 2048);
+	const uint64_t dense_blocks = (uint64_t)b->n_tiles << (b->tile_shift - 6); // 64-position blocks of k_vm_dense
+	ChainOverride force = CHAIN_AUTO;
+	if (const char *e = getenv("GSCAN_CHAIN")) force = *e == '1' ? CHAIN_ON : CHAIN_OFF; // tests: force the chain paths on small inputs / switch them off
+	uint32_t path = plan_resolve(pat->prog, mode, b->n_units, b->bytes, dense_blocks, total_cand, force);
+	if (path != GSCAN_RESOLVE_NONE) {
 		CK(ctx, ctx->ord.ensure((size_t)total_cand));
 		CK(ctx, ctx->unit_start.ensure((size_t)b->n_units + 1));
 		CK(ctx, ctx->unit_out.ensure((size_t)b->n_units + 1));
-		CK(ctx, ctx->blk.ensure((size_t)nb_seg + nb_u + (size_t)(total_cand / 2048 + 2) + 8));
+		// block sums of the largest scan of the call: segments, units, dense blocks or chain nodes (at most what fits in the
+		// tables: four arrays of them); every scan starts at offset 0
+		const uint64_t most = std::max<uint64_t>({(uint64_t)n_segs, (uint64_t)b->n_units, dense ? dense_blocks : 0u,
+		                                          path_chain(path) ? kChainTableBytes / 16 : 0u});
+		CK(ctx, ctx->blk.ensure((size_t)(most / 2048 + 8)));
 		ResolveArgs R;
+		memset(&R, 0, sizeof R);
 		R.tiles = b->d_tiles;
 		R.segs = ctx->segs.p;
 		R.occ = ctx->occ.p;
@@ -910,120 +919,76 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 		R.units = b->d_units;
 		R.n_units = b->n_units;
 		R.ord = ctx->ord.p;
-		R.out = nullptr;
 		R.unit_start = ctx->unit_start.p;
 		R.unit_out = ctx->unit_out.p;
 		R.blk = ctx->blk.p;
 		R.totals = reinterpret_cast<uint32_t *>(ctx->cursor.p + 1);
+		R.path = path;
 		R.mode = mode;
 		R.minlen = (uint32_t)pat->prog.minlen;
 		R.engine = pat->prog.use_vm ? (uint32_t)GSCAN_ENGINE_VM : (uint32_t)pat->prog.kind;
+		R.run_min = (uint32_t)pat->prog.run_min;
+		for (int i = 0; i < 8; i++) R.bitmap[i] = dense ? pat->prog.first_set.w[i] : pat->prog.run_class.w[i];
+		R.total_cand = (uint32_t)total_cand;
 		R.vm_code = ctx->vm_code;
 		R.vm_sets = ctx->vm_sets;
 		R.vm_runstart = pat->prog.vm_runstart ? 1u : 0u;
-		R.flat = (mode == GSCAN_MODE_ALL && !pat->prog.use_vm && (pat->prog.kind == ENGINE_RUN || pat->prog.disjoint)) ? 1u : 0u;
-		// chain path: FIXED patterns whose replay is sequential (overlapping matches, or LINE mode) with many candidates per
-		// unit -- one thread per unit would walk them alone (a 1 GiB window of a log file with a million hits: seconds)
-		R.chain = 0; R.chain_levels = 0; R.chain_cap = 0; R.chain_buf = nullptr;
-		R.vm_par = 0; R.vm_ord = nullptr; R.vm_unit_start = nullptr; R.vm_flag = nullptr; R.vm_budget = nullptr;
-		R.vm_two = 0; R.vm_ord_b = nullptr; R.vm_chain_run = 0; R.vm_limit = R.totals + 2;
-		const bool two = pat->prog.use_vm && !pat->prog.vm_runstart && pat->prog.vm_reach == 1;
-		{
-			// general patterns take the same path when the candidates come from a leading-sequence filter and an attempt's
-			// outcome depends on the search start at most through the attempt's first byte (vm_reach <= 1; reach 1: two
-			// outcomes per candidate, vm_two), or when they are the run starts of a greedy / possessive leading class repeat
-			// (vm_chain_run): the VM attempts of all candidates at once, then the chain over the ones that matched (any mode)
-			// -- instead of one thread replaying a huge unit's attempts alone.  RUN in LINE mode too: the search resumes behind
-			// a line remainder, possibly inside a run (chain_entry)
-			const bool fixed_ok = !pat->prog.use_vm && ((pat->prog.kind == ENGINE_FIXED && (mode == GSCAN_MODE_ALL || mode == GSCAN_MODE_LINE)) ||
-			                                            (pat->prog.kind == ENGINE_RUN && mode == GSCAN_MODE_LINE));
-			const bool run_ok = pat->prog.use_vm && pat->prog.vm_runstart && pat->prog.vm_reach == 0 && pat->prog.vm_lead != VM_Q_LAZY;
-			const bool vm_ok = (pat->prog.use_vm && !pat->prog.vm_runstart && pat->prog.vm_reach <= 1) || run_ok;
-			const bool eligible = !R.flat && !dense && (fixed_ok || vm_ok) && total_cand > 0;
-			bool want = eligible && total_cand >= 65536 && total_cand / std::max<uint64_t>(b->n_units, 1) >= 1024;
-			if (const char *e = getenv("GSCAN_CHAIN")) // tests: force the path on small inputs / switch it off
-				want = eligible && *e == '1';
-			const uint64_t nodes = two ? 2 * total_cand : total_cand;      // vm_two: outcomes A and B of every candidate
-			const uint32_t extra = (two || run_ok) ? 4 : 2;               // marks, ranks (+ the B scan and list / resume points)
-			uint32_t levels = 2; // at least two tables: the second one doubles as the RUN entry positions
-			while ((1ull << levels) < nodes) levels++;
-			if (want && (uint64_t)(levels + extra) * nodes * 4 <= (4ull << 30)) {
-				CK(ctx, ctx->chain.ensure((size_t)(levels + extra) * (size_t)nodes));
-				R.chain = 1; R.chain_levels = levels; R.chain_cap = (uint32_t)nodes; R.chain_buf = ctx->chain.p;
-				if (vm_ok) {
-					CK(ctx, ctx->vm_ord.ensure((size_t)nodes));
-					CK(ctx, ctx->vm_flag.ensure((size_t)nodes));
-					CK(ctx, ctx->vm_unit_start.ensure((size_t)b->n_units + 1));
-					CK(ctx, ctx->vm_budget.ensure((size_t)b->n_units));
-					R.vm_budget = ctx->vm_budget.p;
-					R.vm_par = 1; R.vm_ord = ctx->vm_ord.p; R.vm_flag = ctx->vm_flag.p; R.vm_unit_start = ctx->vm_unit_start.p;
-					R.vm_chain_run = run_ok ? 1u : 0u;
-					if (two) {
-						CK(ctx, ctx->vm_ord_b.ensure((size_t)total_cand));
-						CK(ctx, ctx->blk.ensure((size_t)nb_seg + nb_u + (size_t)(nodes / 2048 + 2) + 8));
-						R.blk = ctx->blk.p;
-						R.vm_two = 1; R.vm_ord_b = ctx->vm_ord_b.p;
-					}
-				}
+		R.vm_dense = dense ? 1u : 0u;
+		R.vm_limit = R.totals + 2;
+		R.dense_tile_shift = b->tile_shift;
+		if (path_vm_chain(path)) {
+			CK(ctx, ctx->vm_budget.ensure((size_t)b->n_units));
+			CK(ctx, ctx->vm_unit_start.ensure((size_t)b->n_units + 1));
+			R.vm_budget = ctx->vm_budget.p;
+			R.vm_unit_start = ctx->vm_unit_start.p;
+		}
+		if (path_chain(path) && !path_compacted(path)) {
+			const ChainGeom g = chain_geom(path, total_cand);
+			CK(ctx, ctx->chain.ensure((size_t)g.arrays * (size_t)g.nodes));
+			R.chain_levels = g.levels; R.chain_cap = (uint32_t)g.nodes; R.chain_buf = ctx->chain.p;
+			if (path_attempts(path)) {
+				CK(ctx, ctx->vm_ord.ensure((size_t)g.nodes));
+				CK(ctx, ctx->vm_flag.ensure((size_t)g.nodes));
+				R.vm_ord = ctx->vm_ord.p; R.vm_flag = ctx->vm_flag.p;
+			}
+			if (path_two(path)) {
+				CK(ctx, ctx->vm_ord_b.ensure((size_t)total_cand));
+				R.vm_ord_b = ctx->vm_ord_b.p;
 			}
 		}
-		R.run_min = (uint32_t)pat->prog.run_min;
-		for (int i = 0; i < 8; i++) R.bitmap[i] = dense ? pat->prog.first_set.w[i] : pat->prog.run_class.w[i];
-		R.vm_dense = dense ? 1u : 0u;
-		R.total_cand = (uint32_t)total_cand;
-		R.vm_ready = 0; R.dense_blocks = 0; R.dense_tile_shift = b->tile_shift;
 		uint32_t nl = 0;
 		uint32_t *h_tot = reinterpret_cast<uint32_t *>((uint8_t *)ctx->readback.p + 16);
 		bool resolved_empty = false;
-		if (dense && pat->prog.vm_reach <= 1) {
+		if (path_compacted(path)) {
 			// dense general pattern, big units: the attempts of all positions in parallel (k_vm_dense, twice: count / write), then
-			// the chain over the matching positions -- one thread per unit would walk a 1 GiB window for minutes
-			const uint64_t blocks = (uint64_t)b->n_tiles << (b->tile_shift - 6);
-			bool want = b->bytes / std::max<uint64_t>(b->n_units, 1) >= (1u << 20);
-			if (const char *e = getenv("GSCAN_CHAIN")) want = *e == '1'; // tests: force the path on small inputs / switch it off
-			if (want && b->bytes <= (4ull << 30) && blocks < (1ull << 31)) {
-				const uint32_t nb_u = (uint32_t)((b->n_units + 2047) / 2048);
-				CK(ctx, ctx->vm_flag.ensure((size_t)blocks + 1));
-				CK(ctx, ctx->vm_budget.ensure((size_t)b->n_units));
-				CK(ctx, ctx->vm_unit_start.ensure((size_t)b->n_units + 1));
-				CK(ctx, ctx->blk.ensure((size_t)(blocks / 2048 + 2) + nb_u + 16));
-				R.blk = ctx->blk.p;
-				R.dense_blocks = (uint32_t)blocks;
-				R.vm_flag = ctx->vm_flag.p; R.vm_budget = ctx->vm_budget.p; R.vm_unit_start = ctx->vm_unit_start.p;
-				R.vm_two = two ? 1u : 0u; // reach 1: both outcomes of every position (the nodes' kinds go beside the chain tables)
-				CK(ctx, launch_vm_dense_count(R, ctx->stream, &nl));
+			// the chain over the matching positions
+			CK(ctx, ctx->vm_flag.ensure((size_t)dense_blocks + 1));
+			R.vm_flag = ctx->vm_flag.p;
+			R.dense_blocks = (uint32_t)dense_blocks;
+			CK(ctx, launch_vm_dense_count(R, ctx->stream, &nl));
+			S.total_launches += nl;
+			uint32_t *h8 = reinterpret_cast<uint32_t *>((uint8_t *)ctx->readback.p + 32);
+			CK(ctx, cudaMemcpyAsync(h8, R.totals, 32, cudaMemcpyDeviceToHost, ctx->stream));
+			CK(ctx, cudaStreamSynchronize(ctx->stream));
+			const uint64_t hits = h8[4];
+			const ChainGeom g = chain_geom(path, hits);
+			if (hits == 0) {
+				h_tot[0] = 0; h_tot[1] = 0; h_tot[2] = h8[2];
+				resolved_empty = true;
+			} else if (g.fits) {
+				CK(ctx, ctx->vm_ord.ensure((size_t)hits));
+				CK(ctx, ctx->chain.ensure((size_t)g.arrays * (size_t)hits));
+				R.vm_ord = ctx->vm_ord.p;
+				R.chain_levels = g.levels; R.chain_cap = (uint32_t)hits; R.chain_buf = ctx->chain.p; // two outcomes: the write pass fills chain_bscan
+				CK(ctx, launch_vm_dense_write(R, ctx->stream, &nl));
 				S.total_launches += nl;
-				uint32_t *h8 = reinterpret_cast<uint32_t *>((uint8_t *)ctx->readback.p + 32);
-				CK(ctx, cudaMemcpyAsync(h8, R.totals, 32, cudaMemcpyDeviceToHost, ctx->stream));
-				CK(ctx, cudaStreamSynchronize(ctx->stream));
-				const uint64_t hits = h8[4];
-				uint32_t levels = 2;
-				while ((1ull << levels) < hits) levels++;
-				if (hits == 0) {
-					h_tot[0] = 0; h_tot[1] = 0; h_tot[2] = h8[2];
-					resolved_empty = true;
-				} else if ((uint64_t)(levels + (two ? 4 : 2)) * hits * 4 <= (4ull << 30)) {
-					CK(ctx, ctx->vm_ord.ensure((size_t)hits));
-					CK(ctx, ctx->chain.ensure((size_t)(levels + (two ? 4 : 2)) * (size_t)hits));
-					CK(ctx, ctx->blk.ensure((size_t)(blocks / 2048 + 2) + nb_u + (size_t)(hits / 2048 + 2) + 16));
-					R.blk = ctx->blk.p;
-					R.vm_ord = ctx->vm_ord.p;
-					R.chain = 1; R.chain_levels = levels; R.chain_cap = (uint32_t)hits; R.chain_buf = ctx->chain.p; // vm_two: the write pass fills chain_bscan
-					CK(ctx, launch_vm_dense_write(R, ctx->stream, &nl));
-					S.total_launches += nl;
-					R.vm_par = 1; R.vm_ready = 1; R.vm_dense = 0;
-					R.total_cand = (uint32_t)hits;
-					S.n_candidates = hits; // matching outcomes (vm_two: A and B counted apart)
-				} else {
-					R.vm_two = 0; // more matching positions than the chain tables may hold -- the per-unit walk below serves the batch
-				}
+				R.total_cand = (uint32_t)hits;
+				S.n_candidates = hits; // matching outcomes (two outcomes: A and B counted apart)
+			} else {
+				path = R.path = GSCAN_RESOLVE_WALK; // more matching positions than the chain tables may hold -- the per-unit walk serves the batch
 			}
 		}
-		S.resolve_path = resolved_empty ? (R.vm_two ? GSCAN_RESOLVE_VM_DENSE_TWO : GSCAN_RESOLVE_VM_DENSE)
-		               : R.vm_chain_run ? GSCAN_RESOLVE_VM_RUN_CHAIN
-		               : R.vm_par ? (R.vm_ready ? (R.vm_two ? GSCAN_RESOLVE_VM_DENSE_TWO : GSCAN_RESOLVE_VM_DENSE)
-		                                        : (R.vm_two ? GSCAN_RESOLVE_VM_TWO : GSCAN_RESOLVE_VM_ATTEMPTS))
-		               : R.chain ? GSCAN_RESOLVE_CHAIN : R.flat ? GSCAN_RESOLVE_FLAT : GSCAN_RESOLVE_WALK;
+		S.resolve_path = path;
 		if (!resolved_empty) {
 			CK(ctx, launch_resolve_count(R, ctx->stream, &nl));
 			S.total_launches += nl;

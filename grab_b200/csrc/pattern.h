@@ -105,9 +105,9 @@ struct Program {
 	ByteSet first_set;             // vm_dense: bytes a match can start with
 	int vm_reach = 0;              // sound upper bound L: an attempt at p has the same outcome for every subject beginning s <= p - L
 	                               // (only ^ \A \b \B (?m)^ and look-behinds near the attempt's first byte look at s; 1: the
-	                               // attempt at s itself differs from "any earlier start", resolve: ResolveArgs::vm_two)
+	                               // attempt at s itself differs from "any earlier start", resolve: GSCAN_RESOLVE_VM_TWO)
 	bool vm_start_free = false;    // vm_reach == 0: an anchored attempt at a position gives the same result wherever the subject
-	                               // begins, so the attempts of a unit's candidates can run in parallel (resolve: ResolveArgs::vm_par)
+	                               // begins, so the attempts of a unit's candidates can run in parallel (resolve: GSCAN_RESOLVE_VM_ATTEMPTS)
 	int vm_lead = 0;               // vm_runstart: VM_Q_* of the leading repeat (after (?U))
 	std::vector<uint32_t> vm_code; // 3 words per instruction
 	std::vector<uint32_t> vm_sets; // 8 words per byte class

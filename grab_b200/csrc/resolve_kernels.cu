@@ -342,7 +342,7 @@ __global__ void k_walk(const ResolveArgs R)
 		const uint64_t ulen = du.len;
 		const bool run = R.engine == GSCAN_ENGINE_RUN;
 		uint64_t start = 0;
-		if (!WRITE && R.flat) {
+		if (!WRITE && R.path == GSCAN_RESOLVE_FLAT) {
 			// ALL mode, no two matches can overlap: every candidate is a match as long as the loop guard start + minlen < ulen
 			// (grab.cc:175, Q1) holds.  Runs never touch each other (a non-class byte separates them), so for RUN it can only
 			// bite before the first search; for FIXED it can also drop the LAST candidate (the one that exactly fills what the
@@ -388,7 +388,7 @@ __global__ void k_walk(const ResolveArgs R)
 	if (!WRITE) R.unit_out[u] = n;
 }
 
-// write pass of the flat case (ResolveArgs::flat): one thread per candidate
+// write pass of GSCAN_RESOLVE_FLAT: one thread per candidate
 __global__ void k_write_flat(const ResolveArgs R)
 {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -415,25 +415,25 @@ __global__ void k_write_flat(const ResolveArgs R)
 	R.out[R.unit_out[c.unit] + idx] = r;
 }
 
-// ---- chain path: the per-unit replay as pointer doubling over all candidates (ResolveArgs::chain) ----
+// ---- chain paths: the per-unit replay as pointer doubling over all candidates (GSCAN_RESOLVE_CHAIN and the VM_* paths) ----
 constexpr uint32_t kChainEnd = 0xffffffffu;
-__device__ __forceinline__ uint32_t *chain_level(const ResolveArgs &R, uint32_t k) { return R.chain_buf + (size_t)k * R.chain_cap; }
-__device__ __forceinline__ uint32_t *chain_mark(const ResolveArgs &R) { return R.chain_buf + (size_t)R.chain_levels * R.chain_cap; }
-__device__ __forceinline__ uint32_t *chain_rank(const ResolveArgs &R) { return R.chain_buf + (size_t)(R.chain_levels + 1) * R.chain_cap; }
-// vm_two: is-B flag of every node, then (in place) its exclusive scan; the B nodes' indices in order.  vm_chain_run: where each
-// node's search resumes, and the outcome of the attempt there (k_vm_resume)
-__device__ __forceinline__ uint32_t *chain_bscan(const ResolveArgs &R) { return R.chain_buf + (size_t)(R.chain_levels + 2) * R.chain_cap; }
+__host__ __device__ __forceinline__ uint32_t *chain_level(const ResolveArgs &R, uint32_t k) { return R.chain_buf + (size_t)k * R.chain_cap; }
+__host__ __device__ __forceinline__ uint32_t *chain_mark(const ResolveArgs &R) { return R.chain_buf + (size_t)R.chain_levels * R.chain_cap; }
+__host__ __device__ __forceinline__ uint32_t *chain_rank(const ResolveArgs &R) { return R.chain_buf + (size_t)(R.chain_levels + 1) * R.chain_cap; }
+// VM_TWO / VM_DENSE_TWO: is-B flag of every node, then (in place) its exclusive scan; the B nodes' indices in order.
+// VM_RUN_CHAIN: where each node's search resumes, and the outcome of the attempt there (k_vm_resume)
+__host__ __device__ __forceinline__ uint32_t *chain_bscan(const ResolveArgs &R) { return R.chain_buf + (size_t)(R.chain_levels + 2) * R.chain_cap; }
 __device__ __forceinline__ uint32_t *chain_blist(const ResolveArgs &R) { return R.chain_buf + (size_t)(R.chain_levels + 3) * R.chain_cap; }
 __device__ __forceinline__ uint32_t *chain_stop(const ResolveArgs &R) { return chain_bscan(R); }
 __device__ __forceinline__ uint32_t *chain_resume(const ResolveArgs &R) { return chain_blist(R); }
 
-// vm_two, chain view (totals[0]: nodes, totals[1]: B nodes): node j is a B node when the exclusive count steps behind it
+// two outcomes, chain view (totals[0]: nodes, totals[1]: B nodes): node j is a B node when the exclusive count steps behind it
 __device__ __forceinline__ bool two_is_b(const ResolveArgs &R, uint32_t j)
 {
 	const uint32_t *bs = chain_bscan(R);
 	return (j + 1 < R.totals[0] ? bs[j + 1] : R.totals[1]) != bs[j];
 }
-// vm_two: where a search that resumes at `s` goes on -- lo: the unit's first node at or after s, uend: the unit's end.  Node
+// two outcomes: where a search that resumes at `s` goes on -- lo: the unit's first node at or after s, uend: the unit's end.  Node
 // (s, A) if A(s) matched; else the first B node behind s (B(s) itself is never taken: the subject began AT s)
 __device__ __forceinline__ uint32_t two_next(const ResolveArgs &R, uint32_t lo, uint32_t uend, uint64_t s)
 {
@@ -453,7 +453,7 @@ __global__ void k_chain_next(const ResolveArgs R)
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= R.totals[0]) return;
 	const OutRec c = R.ord[i];
-	if (R.vm_par && c.pad >= 2u) { chain_level(R, 0)[i] = kChainEnd; return; } // this match ends its unit's loop (Q2 / VM limit)
+	if (path_vm_chain(R.path) && c.pad >= 2u) { chain_level(R, 0)[i] = kChainEnd; return; } // this match ends its unit's loop (Q2 / VM limit)
 	const DevUnit du = R.units[c.unit];
 	const uint64_t ulen = du.len;
 	const uint8_t *data = reinterpret_cast<const uint8_t *>(du.ptr);
@@ -471,25 +471,25 @@ __global__ void k_chain_next(const ResolveArgs R)
 	}
 	if (run) R.ord[i].pad = (uint32_t)stop; // where the search resumes behind this match (k_chain_entry)
 	uint32_t nx = kChainEnd;
-	if (R.vm_chain_run && chain_resume(R)[i] == 2u) stop = ulen; // the attempt where the search resumes ran into the VM limit
+	if (path_run(R.path) && chain_resume(R)[i] == 2u) stop = ulen; // the attempt where the search resumes ran into the VM limit
 	if (stop + R.minlen < ulen) {
 		// RUN: the search may resume INSIDE a run (behind a line remainder); if what is left of that run is long enough the
 		// leftmost match is at `stop` itself -- it ends where the run's own candidate ends, so the chain goes on from that
-		// candidate and only the reported start differs (chain_entry).  vm_chain_run: k_vm_resume ran the attempt there
+		// candidate and only the reported start differs (chain_entry).  VM_RUN_CHAIN: k_vm_resume ran the attempt there
 		bool inside = false;
 		if (run && stop > 0 && in_class(R, data[stop - 1]) && in_class(R, data[stop])) {
 			uint64_t e = stop;
 			while (e < ulen && in_class(R, data[e])) e++;
 			inside = e - stop >= R.run_min;
 		}
-		if (R.vm_chain_run) inside = chain_resume(R)[i] == 1u;
+		if (path_run(R.path)) inside = chain_resume(R)[i] == 1u;
 		const uint32_t uend = R.unit_start[c.unit + 1];
 		uint32_t lo = i + 1, hi = uend; // candidates are ordered by position inside the unit
 		while (lo < hi) {
 			const uint32_t mid = lo + ((hi - lo) >> 1);
 			if (R.ord[mid].pos < stop) lo = mid + 1; else hi = mid;
 		}
-		if (R.vm_two) nx = two_next(R, lo, uend, stop);
+		if (path_two(R.path)) nx = two_next(R, lo, uend, stop);
 		else if (inside) nx = lo > i + 1 ? lo - 1 : kChainEnd; // the run that holds `stop`: the last one that starts before it (behind i's own run)
 		else if (lo < uend) nx = lo;
 	}
@@ -513,7 +513,7 @@ __global__ void k_chain_heads(const ResolveArgs R)
 	if (u >= R.n_units) return;
 	const uint32_t first = R.unit_start[u], end = R.unit_start[u + 1];
 	if (first == end || !(R.minlen < (uint64_t)R.units[u].len)) return;
-	const uint32_t h = R.vm_two ? two_next(R, first, end, 0u) : first; // vm_two: the first search begins at 0
+	const uint32_t h = path_two(R.path) ? two_next(R, first, end, 0u) : first; // two outcomes: the first search begins at 0
 	if (h != kChainEnd) chain_mark(R)[h] = 1u;
 }
 
@@ -544,11 +544,11 @@ __global__ void k_chain_entry(const ResolveArgs R)
 	if (!chain_mark(R)[i]) return;
 	const uint32_t nx = chain_level(R, 0)[i];
 	if (nx == kChainEnd) return;
-	const uint32_t stop = R.vm_chain_run ? chain_stop(R)[i] : R.ord[i].pad;
+	const uint32_t stop = path_run(R.path) ? chain_stop(R)[i] : R.ord[i].pad;
 	if (stop > R.ord[nx].pos) chain_entry(R)[nx] = stop; // one marked predecessor per chain member: no two writers
 }
 
-// vm_par: a candidate that ends its unit's loop (pad 2: a capturing group was set, pcre_exec returns 0; pad 3: VM limit,
+// VM_* paths: a candidate that ends its unit's loop (pad 2: a capturing group was set, pcre_exec returns 0; pad 3: VM limit,
 // pcre_exec returns an error) is on the chain -- nothing behind it is -- but is not a reported match
 __global__ void k_chain_unmark(const ResolveArgs R)
 {
@@ -576,7 +576,7 @@ __global__ void k_chain_write(const ResolveArgs R)
 	const OutRec c = R.ord[i];
 	const DevUnit du = R.units[c.unit];
 	const uint32_t k = chain_rank(R)[i] - chain_rank(R)[R.unit_start[c.unit]];
-	const uint32_t from = (R.engine == GSCAN_ENGINE_RUN || R.vm_chain_run) ? chain_entry(R)[i] : c.pos;
+	const uint32_t from = (R.engine == GSCAN_ENGINE_RUN || path_run(R.path)) ? chain_entry(R)[i] : c.pos;
 	FinalRec r;
 	r.start = du.base_off + from;
 	r.file_id = du.file_id;
@@ -584,7 +584,7 @@ __global__ void k_chain_write(const ResolveArgs R)
 	R.out[R.unit_out[c.unit] + k] = r;
 }
 
-// ---- general patterns on the chain path (ResolveArgs::vm_par) ----
+// ---- general patterns on the chain paths (GSCAN_RESOLVE_VM_*) ----
 // One anchored attempt per candidate, every candidate of the batch at once.  The subject of the attempt begins at the
 // candidate itself: for a start-free program (no ^, \A, \b, \B, (?m)^, look-behind) the result is the one pcre_exec
 // reaches from any search start at or before the candidate (grab.cc:178).
@@ -602,8 +602,8 @@ __global__ void __launch_bounds__(64, 4) k_vm_attempts(const ResolveArgs R)
 	if (rc < 0) { atomicOr(R.totals + 2, 1u); rc = 3; }
 	R.ord[i].len = e;             // the subject began at the candidate: the end offset is the match length
 	R.ord[i].pad = (uint32_t)rc;  // 0: no match here, 1: match, 2: match with a capturing group set (Q2), 3: VM limit
-	if (!R.vm_two) { R.vm_flag[i] = rc != 0 ? 1u : 0u; return; }
-	// vm_two: B(p), the subject begins one byte before the candidate -- what every earlier search start sees (reach 1)
+	if (!path_two(R.path)) { R.vm_flag[i] = rc != 0 ? 1u : 0u; return; }
+	// VM_TWO: B(p), the subject begins one byte before the candidate -- what every earlier search start sees (reach 1)
 	OutRec b;
 	b.unit = c.unit; b.pos = c.pos; b.len = 0; b.pad = 0;
 	if (c.pos >= 1u) {
@@ -620,23 +620,23 @@ __global__ void __launch_bounds__(64, 4) k_vm_attempts(const ResolveArgs R)
 	R.vm_flag[2 * i + 1] = b.pad != 0 ? 1u : 0u;
 }
 
-// vm_two / vm_chain_run: the budget covers two attempts per position (A and B; a run start and a search resuming inside its
+// two outcomes / VM_RUN_CHAIN: the budget covers two attempts per position (A and B; a run start and a search resuming inside its
 // run), twice what the serial walk gets -- it makes one attempt per position and search
 __global__ void k_vm_budget_init(const ResolveArgs R)
 {
 	const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
 	if (u >= R.n_units) return;
-	R.vm_budget[u] = VmBudget::unit_total(R.units[u].len) << ((R.vm_two || R.vm_chain_run) ? 1 : 0);
+	R.vm_budget[u] = VmBudget::unit_total(R.units[u].len) << ((path_two(R.path) || path_run(R.path)) ? 1 : 0);
 }
 
-// vm_flag holds its own exclusive scan by now: the candidates that matched, in order (vm_two: A then B of every candidate,
+// vm_flag holds its own exclusive scan by now: the candidates that matched, in order (VM_TWO: A then B of every candidate,
 // and the node's kind into chain_bscan)
 __global__ void k_vm_compact(const ResolveArgs R)
 {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= R.totals[0]) return;
 	const OutRec c = R.ord[i];
-	if (!R.vm_two) {
+	if (!path_two(R.path)) {
 		if (c.pad) R.vm_ord[R.vm_flag[i]] = c;
 		return;
 	}
@@ -651,10 +651,10 @@ __global__ void k_vm_unit_starts(const ResolveArgs R)
 	const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
 	if (u > R.n_units) return;
 	const uint32_t s = R.unit_start[u];
-	R.vm_unit_start[u] = s < R.totals[0] ? R.vm_flag[R.vm_two ? 2 * s : s] : R.totals[4];
+	R.vm_unit_start[u] = s < R.totals[0] ? R.vm_flag[path_two(R.path) ? 2 * s : s] : R.totals[4];
 }
 
-// vm_two, chain view, chain_bscan scanned: the index of every B node at its rank among them
+// two outcomes, chain view, chain_bscan scanned: the index of every B node at its rank among them
 __global__ void k_two_blist(const ResolveArgs R)
 {
 	const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -662,7 +662,7 @@ __global__ void k_two_blist(const ResolveArgs R)
 	if (two_is_b(R, j)) chain_blist(R)[chain_bscan(R)[j]] = j;
 }
 
-// vm_chain_run, chain view: where the search resumes behind node i, and -- when that lies inside a run of the leading class
+// VM_RUN_CHAIN, chain view: where the search resumes behind node i, and -- when that lies inside a run of the leading class
 // (the test of k_walk_vm) -- the attempt there: 1 match (it ends where the run start's own match ends: a greedy or possessive
 // C{n,} from inside the run tries a subset of the run start's split points, in the same order), 0 none, 2 VM limit.  Own
 // kernel: the VM's thread-local stack stays out of the chain kernels
@@ -693,7 +693,7 @@ __global__ void __launch_bounds__(64, 4) k_vm_resume(const ResolveArgs R)
 	chain_resume(R)[i] = res;
 }
 
-// ---- dense general patterns on the chain path (ResolveArgs::vm_ready) ----
+// ---- dense general patterns on the chain path (GSCAN_RESOLVE_VM_DENSE*) ----
 // No candidate list: every position whose byte can start a match gets its anchored attempt (what pcre_exec's own search
 // loop does, grab.cc:178), 64 consecutive positions per thread, all blocks of the batch at once.  The count pass leaves the
 // number of matching positions per block in vm_flag; after the exclusive scan the write pass replays the attempts and
@@ -718,9 +718,9 @@ __global__ void __launch_bounds__(64, 4) k_vm_dense(const ResolveArgs R)
 		const uint32_t ulen = du.len;
 		const uint32_t hi = lo + (1u << kDenseShift) < tile_end ? lo + (1u << kDenseShift) : tile_end;
 		VmBudget budget(ulen, R.vm_budget + td.unit);
-		// vm_two: both outcomes of every position, A (subject begins at pos) before B (subject begins at pos - 1); the write
+		// VM_DENSE_TWO: both outcomes of every position, A (subject begins at pos) before B (subject begins at pos - 1); the write
 		// pass records each node's kind in chain_bscan
-		const uint32_t kinds = R.vm_two ? 2u : 1u;
+		const uint32_t kinds = path_two(R.path) ? 2u : 1u;
 		for (uint32_t pos = lo; pos < hi && !(WRITE && n == cnt); pos++) {
 			if ((uint64_t)pos + R.minlen > ulen) break;                                 // an attempt with fewer bytes left cannot succeed
 			if (!in_class(R, data[pos])) continue;
@@ -736,7 +736,7 @@ __global__ void __launch_bounds__(64, 4) k_vm_dense(const ResolveArgs R)
 					OutRec r;
 					r.unit = td.unit; r.pos = pos; r.len = rc == 3 ? 0u : e - k; r.pad = (uint32_t)rc;
 					o[n] = r;
-					if (R.vm_two) chain_bscan(R)[R.vm_flag[b] + n] = k;
+					if (path_two(R.path)) chain_bscan(R)[R.vm_flag[b] + n] = k;
 				}
 				n++;
 			}
@@ -744,7 +744,7 @@ __global__ void __launch_bounds__(64, 4) k_vm_dense(const ResolveArgs R)
 		budget.give_back();
 		if (WRITE) for (; n < cnt; n++) {
 			OutRec r; r.unit = td.unit; r.pos = hi - 1u; r.len = 0; r.pad = 3u; o[n] = r;
-			if (R.vm_two) chain_bscan(R)[R.vm_flag[b] + n] = 1u; // keeps the (pos, A before B) order
+			if (path_two(R.path)) chain_bscan(R)[R.vm_flag[b] + n] = 1u; // keeps the (pos, A before B) order
 		}
 	}
 	if (!WRITE) R.vm_flag[b] = n;
@@ -880,6 +880,103 @@ __global__ void __launch_bounds__(64, 4) k_walk_vm(const ResolveArgs R)
 	if (!WRITE) R.unit_out[u] = n;
 }
 
+// ---- the resolve launch sequence, written once over an executor X ----
+// The device runs it through DeviceExec (launch_* below); the CPU model checks (tests/model_host.h) run the same
+// sequence with every thread id in turn.  X provides
+//   launch(kernel, threads, block, args...)  one thread per index in [0, threads), blocks of `block`
+//   exclusive_scan(v, n, total_out)          in place; the sum of all n values into *total_out
+//   fill_zero(p, n), copy(dst, src, n)       u32 words
+// what the chain kernels see: the candidate list itself, or (VM_* paths) the compacted list of the outcomes that matched with
+// its own count (totals[4]) and rank-total scratch (totals[7])
+inline ResolveArgs chain_view(const ResolveArgs &R)
+{
+	ResolveArgs C = R;
+	if (path_vm_chain(R.path)) { C.ord = R.vm_ord; C.unit_start = R.vm_unit_start; C.totals = R.totals + 4; }
+	return C;
+}
+
+// count pass, behind the gather (VM_DENSE*: behind vm_dense_write): per-unit match counts into unit_out, their exclusive
+// scan (the output slots), totals[1] = number of matches
+template <class X>
+void resolve_count_seq(X &x, const ResolveArgs &R)
+{
+	if (path_chain(R.path)) {
+		// grids cover the reserved node slots; the kernels stop at the exact count (totals[0], on the device by now)
+		const uint32_t cap = R.chain_cap;
+		if (path_attempts(R.path)) {
+			x.fill_zero(R.vm_flag, cap); // VM_TWO: cap is two slots per candidate
+			if (path_two(R.path)) x.fill_zero(chain_bscan(R), cap);
+			x.launch(k_vm_budget_init, R.n_units, 256, R);
+			x.launch(k_vm_attempts, cap, 64, R);
+			x.exclusive_scan(R.vm_flag, cap, R.totals + 4);
+			x.launch(k_vm_compact, cap, 256, R);
+			x.launch(k_vm_unit_starts, R.n_units + 1, 256, R);
+		}
+		const ResolveArgs C = chain_view(R);
+		if (path_two(R.path)) { // which nodes are B: exclusive count (total: totals[5]) and the list of their indices
+			x.exclusive_scan(chain_bscan(C), cap, R.totals + 5);
+			x.launch(k_two_blist, cap, 256, C);
+		}
+		const bool follow = R.mode != GSCAN_MODE_FIRST; // FIRST: the head of every unit's chain is all there is
+		x.fill_zero(chain_mark(C), cap);                // (the ranks are a copy of the marks, below)
+		if (follow) {
+			if (path_run(R.path)) x.launch(k_vm_resume, cap, 64, C);
+			x.launch(k_chain_next, cap, 256, C);
+			for (uint32_t k = 1; k < C.chain_levels; k++) x.launch(k_chain_double, cap, 256, C, k);
+		}
+		x.launch(k_chain_heads, R.n_units, 256, C);
+		if (follow) for (uint32_t k = C.chain_levels; k-- > 0;) x.launch(k_chain_spread, cap, 256, C, k);
+		if (path_vm_chain(R.path)) x.launch(k_chain_unmark, cap, 256, C);
+		if (R.engine == GSCAN_ENGINE_RUN || path_run(R.path)) {
+			x.launch(k_chain_entry_init, cap, 256, C);
+			if (follow) x.launch(k_chain_entry, cap, 256, C);
+		}
+		x.copy(chain_rank(C), chain_mark(C), cap);
+		x.exclusive_scan(chain_rank(C), cap, C.totals + 3);
+		x.launch(k_chain_count, R.n_units, 256, C);
+	} else if (R.engine == GSCAN_ENGINE_VM) {
+		x.launch(k_walk_vm<false>, R.n_units, 64, R);
+	} else {
+		x.launch(k_walk<false>, R.n_units, 128, R);
+	}
+	x.exclusive_scan(R.unit_out, R.n_units, R.totals + 1);
+}
+
+// VM_DENSE*: the matching positions per 64-position block into vm_flag, exclusive scan, total into totals[4]
+template <class X>
+void vm_dense_count_seq(X &x, const ResolveArgs &R)
+{
+	x.launch(k_vm_budget_init, R.n_units, 256, R);
+	x.launch(k_vm_dense<false>, R.dense_blocks, 64, R);
+	x.exclusive_scan(R.vm_flag, R.dense_blocks, R.totals + 4);
+}
+
+// VM_DENSE*, once vm_ord and the chain tables are sized: the node list and vm_unit_start
+template <class X>
+void vm_dense_write_seq(X &x, const ResolveArgs &R)
+{
+	x.launch(k_vm_budget_init, R.n_units, 256, R);
+	x.launch(k_vm_dense<true>, R.dense_blocks, 64, R);
+	x.launch(k_vm_dense_unit_starts, R.n_units + 1, 256, R);
+}
+
+// write pass: the records into R.out, at the slots of the count pass
+template <class X>
+void resolve_write_seq(X &x, const ResolveArgs &R)
+{
+	if (path_chain(R.path)) {
+		ResolveArgs C = chain_view(R);
+		if (path_two(R.path)) C.total_cand = R.chain_cap; // two node slots per candidate; the slots behind the nodes are unmarked
+		x.launch(k_chain_write, C.total_cand, 256, C);
+	} else if (R.path == GSCAN_RESOLVE_FLAT) {
+		x.launch(k_write_flat, R.total_cand, 256, R);
+	} else if (R.engine == GSCAN_ENGINE_VM) {
+		x.launch(k_walk_vm<true>, R.n_units, 64, R);
+	} else {
+		x.launch(k_walk<true>, R.n_units, 128, R);
+	}
+}
+
 // ---- 4. generic u32 block sums / exclusive scan (per-unit match counts -> output slots) ----
 __global__ void k_u32_sums(const uint32_t *v, uint32_t n, uint32_t *blk)
 {
@@ -913,120 +1010,78 @@ __global__ void k_fill_zero(uint32_t *p, uint32_t n)
 	if (i < n) p[i] = 0u;
 	if (i + gridDim.x * blockDim.x < n) p[i + gridDim.x * blockDim.x] = 0u;
 }
-static uint32_t *chain_mark_host(const ResolveArgs &R) { return R.chain_buf + (size_t)R.chain_levels * R.chain_cap; }
-// what the chain kernels see: the candidate list itself, or (vm_par) the compacted list of the candidates that matched with
-// its own count (totals[4]) and rank-total scratch (totals[7])
-static ResolveArgs chain_view(const ResolveArgs &R)
-{
-	ResolveArgs C = R;
-	if (R.vm_par) { C.ord = R.vm_ord; C.unit_start = R.vm_unit_start; C.totals = R.totals + 4; }
-	return C;
-}
+// the executor of the launch sequence on the device: the grids cover `threads` in blocks of `block`; every scan is
+// k_u32_sums -> k_scan_blk -> k_u32_exclusive with its block sums in R.blk from offset 0 (the stream orders the scans)
+struct DeviceExec {
+	cudaStream_t st;
+	uint32_t *blk;
+	uint32_t launches = 0;
+	cudaError_t err = cudaSuccess;
+	template <class... P, class... A>
+	void launch(void (*kernel)(P...), uint32_t threads, uint32_t block, A... args)
+	{
+		kernel<<<(threads + block - 1) / block, block, 0, st>>>(args...);
+		launches++;
+	}
+	void exclusive_scan(uint32_t *v, uint32_t n, uint32_t *total_out)
+	{
+		const uint32_t nb = (n + kPerBlock - 1) / kPerBlock;
+		k_u32_sums<<<nb, kScanBlock, 0, st>>>(v, n, blk);
+		k_scan_blk<<<1, kScanBlock, 0, st>>>(blk, nb, total_out, nullptr);
+		k_u32_exclusive<<<nb, kScanBlock, 0, st>>>(v, n, blk);
+		launches += 3;
+	}
+	void fill_zero(uint32_t *p, uint32_t n)
+	{
+		k_fill_zero<<<(n + 255) / 256, 256, 0, st>>>(p, n);
+		launches++;
+	}
+	void copy(uint32_t *dst, const uint32_t *src, uint32_t n)
+	{
+		const cudaError_t e = cudaMemcpyAsync(dst, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, st);
+		if (err == cudaSuccess) err = e;
+	}
+	cudaError_t finish(uint32_t *n_launches)
+	{
+		if (n_launches) *n_launches = launches;
+		const cudaError_t e = cudaGetLastError();
+		return err != cudaSuccess ? err : e;
+	}
+};
 
 cudaError_t launch_resolve_count(const ResolveArgs &R, cudaStream_t st, uint32_t *launches)
 {
-	uint32_t nl = 0;
-	const uint32_t nb_seg = (R.vm_dense || R.vm_ready) ? 0u : (R.n_segs + kPerBlock - 1) / kPerBlock;
-	if (!R.vm_dense && !R.vm_ready) {
-		k_seg_sums<<<nb_seg, kScanBlock, 0, st>>>(R.segs, R.occ, R.n_segs, R.tag, R.blk); nl++;
-		k_scan_blk<<<1, kScanBlock, 0, st>>>(R.blk, nb_seg, R.totals, R.unit_start + R.n_units); nl++;
-		k_gather<<<nb_seg, kScanBlock, 0, st>>>(R); nl++;
+	DeviceExec x{st, R.blk};
+	if (!R.vm_dense) { // segment prefix sum and gather; k_gather reads the segment scan's block sums
+		const uint32_t nb_seg = (R.n_segs + kPerBlock - 1) / kPerBlock;
+		k_seg_sums<<<nb_seg, kScanBlock, 0, st>>>(R.segs, R.occ, R.n_segs, R.tag, R.blk);
+		k_scan_blk<<<1, kScanBlock, 0, st>>>(R.blk, nb_seg, R.totals, R.unit_start + R.n_units);
+		k_gather<<<nb_seg, kScanBlock, 0, st>>>(R);
+		x.launches += 3;
 	}
-	const uint32_t nb_u = (R.n_units + kPerBlock - 1) / kPerBlock;
-	uint32_t *blk2 = R.blk + nb_seg + 1; // block sums of the per-unit counts live behind the segment block sums
-	if (R.chain) {
-		// grids cover the reserved candidate slots; the kernels stop at the exact count (totals[0], on the device by now)
-		const uint32_t nb_c = (R.chain_cap + 255) / 256, nb_cs = (R.chain_cap + kPerBlock - 1) / kPerBlock;
-		uint32_t *blk3 = blk2 + nb_u + 1;
-		uint32_t *bscan = chain_mark_host(R) + 2u * (size_t)R.chain_cap; // vm_two: chain_bscan
-		if (R.vm_par && !R.vm_ready) {
-			k_fill_zero<<<nb_c, 256, 0, st>>>(R.vm_flag, R.chain_cap); nl++; // vm_two: chain_cap is two slots per candidate
-			if (R.vm_two) { k_fill_zero<<<nb_c, 256, 0, st>>>(bscan, R.chain_cap); nl++; }
-			k_vm_budget_init<<<(R.n_units + 255) / 256, 256, 0, st>>>(R); nl++;
-			k_vm_attempts<<<(R.chain_cap + 63) / 64, 64, 0, st>>>(R); nl++;
-			k_u32_sums<<<nb_cs, kScanBlock, 0, st>>>(R.vm_flag, R.chain_cap, blk3); nl++;
-			k_scan_blk<<<1, kScanBlock, 0, st>>>(blk3, nb_cs, R.totals + 4, nullptr); nl++;
-			k_u32_exclusive<<<nb_cs, kScanBlock, 0, st>>>(R.vm_flag, R.chain_cap, blk3); nl++;
-			k_vm_compact<<<nb_c, 256, 0, st>>>(R); nl++;
-			k_vm_unit_starts<<<(R.n_units + 1 + 255) / 256, 256, 0, st>>>(R); nl++;
-		}
-		const ResolveArgs C = chain_view(R);
-		if (R.vm_two) { // which nodes are B: exclusive count (total: totals[5]) and the list of their indices
-			k_u32_sums<<<nb_cs, kScanBlock, 0, st>>>(bscan, C.chain_cap, blk3); nl++;
-			k_scan_blk<<<1, kScanBlock, 0, st>>>(blk3, nb_cs, R.totals + 5, nullptr); nl++;
-			k_u32_exclusive<<<nb_cs, kScanBlock, 0, st>>>(bscan, C.chain_cap, blk3); nl++;
-			k_two_blist<<<nb_c, 256, 0, st>>>(C); nl++;
-		}
-		const bool follow = R.mode != GSCAN_MODE_FIRST; // FIRST: the head of every unit's chain is all there is
-		k_fill_zero<<<nb_c, 256, 0, st>>>(chain_mark_host(C), 2u * C.chain_cap); nl++; // marks and ranks
-		if (follow) {
-			if (R.vm_chain_run) { k_vm_resume<<<(C.chain_cap + 63) / 64, 64, 0, st>>>(C); nl++; }
-			k_chain_next<<<nb_c, 256, 0, st>>>(C); nl++;
-			for (uint32_t k = 1; k < C.chain_levels; k++) { k_chain_double<<<nb_c, 256, 0, st>>>(C, k); nl++; }
-		}
-		k_chain_heads<<<(C.n_units + 255) / 256, 256, 0, st>>>(C); nl++;
-		if (follow) for (uint32_t k = C.chain_levels; k-- > 0;) { k_chain_spread<<<nb_c, 256, 0, st>>>(C, k); nl++; }
-		if (R.vm_par) { k_chain_unmark<<<nb_c, 256, 0, st>>>(C); nl++; }
-		if (R.engine == GSCAN_ENGINE_RUN || R.vm_chain_run) {
-			k_chain_entry_init<<<nb_c, 256, 0, st>>>(C); nl++;
-			if (follow) { k_chain_entry<<<nb_c, 256, 0, st>>>(C); nl++; }
-		}
-		cudaMemcpyAsync(chain_mark_host(C) + C.chain_cap, chain_mark_host(C), (size_t)C.chain_cap * 4, cudaMemcpyDeviceToDevice, st);
-		k_u32_sums<<<nb_cs, kScanBlock, 0, st>>>(chain_mark_host(C) + C.chain_cap, C.chain_cap, blk3); nl++;
-		k_scan_blk<<<1, kScanBlock, 0, st>>>(blk3, nb_cs, C.totals + 3, nullptr); nl++;
-		k_u32_exclusive<<<nb_cs, kScanBlock, 0, st>>>(chain_mark_host(C) + C.chain_cap, C.chain_cap, blk3); nl++;
-		k_chain_count<<<(C.n_units + 255) / 256, 256, 0, st>>>(C); nl++;
-	} else {
-		if (R.engine == GSCAN_ENGINE_VM) k_walk_vm<false><<<(R.n_units + 63) / 64, 64, 0, st>>>(R);
-		else k_walk<false><<<(R.n_units + 127) / 128, 128, 0, st>>>(R);
-		nl++;
-	}
-	k_u32_sums<<<nb_u, kScanBlock, 0, st>>>(R.unit_out, R.n_units, blk2); nl++;
-	k_scan_blk<<<1, kScanBlock, 0, st>>>(blk2, nb_u, R.totals + 1, nullptr); nl++;
-	k_u32_exclusive<<<nb_u, kScanBlock, 0, st>>>(R.unit_out, R.n_units, blk2); nl++;
-	if (launches) *launches = nl;
-	return cudaGetLastError();
+	resolve_count_seq(x, R);
+	return x.finish(launches);
 }
 
 cudaError_t launch_vm_dense_count(const ResolveArgs &R, cudaStream_t st, uint32_t *launches)
 {
-	const uint32_t nb = (R.dense_blocks + kPerBlock - 1) / kPerBlock;
-	k_vm_budget_init<<<(R.n_units + 255) / 256, 256, 0, st>>>(R);
-	k_vm_dense<false><<<(R.dense_blocks + 63) / 64, 64, 0, st>>>(R);
-	k_u32_sums<<<nb, kScanBlock, 0, st>>>(R.vm_flag, R.dense_blocks, R.blk);
-	k_scan_blk<<<1, kScanBlock, 0, st>>>(R.blk, nb, R.totals + 4, nullptr);
-	k_u32_exclusive<<<nb, kScanBlock, 0, st>>>(R.vm_flag, R.dense_blocks, R.blk);
-	if (launches) *launches = 5;
-	return cudaGetLastError();
+	DeviceExec x{st, R.blk};
+	vm_dense_count_seq(x, R);
+	return x.finish(launches);
 }
 
 cudaError_t launch_vm_dense_write(const ResolveArgs &R, cudaStream_t st, uint32_t *launches)
 {
-	k_vm_budget_init<<<(R.n_units + 255) / 256, 256, 0, st>>>(R);
-	k_vm_dense<true><<<(R.dense_blocks + 63) / 64, 64, 0, st>>>(R);
-	k_vm_dense_unit_starts<<<(R.n_units + 1 + 255) / 256, 256, 0, st>>>(R);
-	if (launches) *launches = 3;
-	return cudaGetLastError();
+	DeviceExec x{st, R.blk};
+	vm_dense_write_seq(x, R);
+	return x.finish(launches);
 }
 
 cudaError_t launch_resolve_write(const ResolveArgs &R, cudaStream_t st, uint32_t *launches)
 {
-	if (R.chain) {
-		ResolveArgs C = chain_view(R);
-		if (R.vm_two) C.total_cand = R.chain_cap; // two node slots per candidate; the slots behind the nodes are unmarked
-		k_chain_write<<<(C.total_cand + 255) / 256, 256, 0, st>>>(C);
-		if (launches) *launches = 1;
-		return cudaGetLastError();
-	}
-	if (R.flat) {
-		k_write_flat<<<(R.total_cand + 255) / 256, 256, 0, st>>>(R);
-		if (launches) *launches = 1;
-		return cudaGetLastError();
-	}
-	if (R.engine == GSCAN_ENGINE_VM) k_walk_vm<true><<<(R.n_units + 63) / 64, 64, 0, st>>>(R);
-	else k_walk<true><<<(R.n_units + 127) / 128, 128, 0, st>>>(R);
-	if (launches) *launches = 1;
-	return cudaGetLastError();
+	DeviceExec x{st, R.blk};
+	resolve_write_seq(x, R);
+	return x.finish(launches);
 }
 
 } // namespace gscan

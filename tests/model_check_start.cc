@@ -1,57 +1,27 @@
 // model_check_start.cc -- CPU check of the resolve paths for general patterns whose attempts look at or before their first
-// byte (Program::vm_reach) and of class-repeat-led patterns (Program::vm_runstart), with the device's own source (the VM and
-// the chain kernels of resolve_kernels.cu, extracted by tests/test_model_start.py) compiled for the host:
+// byte (Program::vm_reach) and of class-repeat-led patterns (Program::vm_runstart), with the device's own source (the VM, the
+// resolve kernels and their launch sequence in resolve_kernels.cu, extracted by tests/test_model_start.py, model_host.h)
+// compiled for the host:
 //   1. reach soundness: an attempt at p gives the same outcome from every subject beginning s <= p - vm_reach; and the check
 //      catches a reach reported one too small (it must find a disagreement for patterns whose reach is exact)
-//   2. reach-1 programs, two outcomes per candidate (vm_two): filtered (k_vm_attempts) and dense (k_vm_dense), then the chain
-//   3. greedy / possessive class-repeat-led programs on the chain (vm_chain_run, k_vm_resume)
+//   2. reach-1 programs, two outcomes per candidate: filtered (VM_TWO, k_vm_attempts) and dense (VM_DENSE_TWO, k_vm_dense),
+//      then the chain
+//   3. greedy / possessive class-repeat-led programs on the chain (VM_RUN_CHAIN, k_vm_resume)
 // against the oracle's loop in all three modes (ALL / FIRST / LINE), for single units and two-unit batches, with and without
 // the capturing-group quirk (Q2, STRICT_REF).
 // Usage: model_check_start PATTERN_FILE   (one pattern per line)
-#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
-#include <cstring>
 #include <fstream>
 #include <string>
-#include <vector>
 
-#include "../include/gscan.h"
-#include "../grab_b200/csrc/pattern.h"
-#include "../grab_b200/csrc/kernels.h"
+#include "model_host.h"
 extern "C" {
 #include "../oracle/grab_oracle.h"
 }
 
-#undef __device__
-#undef __global__
-#undef __forceinline__
-#undef __launch_bounds__
-#define __device__
-#define __global__
-#define __forceinline__ inline
-#define __launch_bounds__(...)
-namespace gscan {
-struct ModelIdx { uint32_t x; };
-static ModelIdx model_blockIdx{0}, model_blockDim{1}, model_threadIdx{0};
-#define blockIdx model_blockIdx
-#define blockDim model_blockDim
-#define threadIdx model_threadIdx
-static inline uint32_t atomicOr(uint32_t *p, uint32_t v) { const uint32_t o = *p; *p |= v; return o; }
-static inline unsigned long long atomicAdd(unsigned long long *p, unsigned long long v) { const unsigned long long o = *p; *p += v; return o; }
-#include "vm_snippet.inc"
-#undef blockIdx
-#undef blockDim
-#undef threadIdx
-} // namespace gscan
-
-using namespace gscan;
-
 static uint64_t rng_state = 0x9e3779b97f4a7c15ull;
 static uint32_t rnd() { rng_state ^= rng_state << 13; rng_state ^= rng_state >> 7; rng_state ^= rng_state << 17; return (uint32_t)(rng_state >> 9); }
-
-struct M { uint64_t pos; uint32_t len; };
-typedef std::vector<uint8_t> Bytes;
 
 // steps an attempt, or all attempts of a unit together, may take here: pathological patterns of the random grammar end in the
 // VM limit (those checks are skipped) in milliseconds instead of seconds
@@ -94,158 +64,17 @@ static long reach_violations(const Program &p, const std::vector<Bytes> &subject
 }
 
 // ---- 2./3. the chain paths ----
-static bool seq_at(const Sequence &q, const uint8_t *s, size_t len, size_t pos)
-{
-	if (pos + q.size() > len) return false;
-	for (size_t i = 0; i < q.size(); i++) if (!q[i].has(s[pos + i])) return false;
-	return true;
-}
-
-// what the scan kernels deliver by contract: leading-sequence hits, or the first byte of every class run >= run_min
-static void candidates(const Program &p, const Bytes &b, uint32_t unit, std::vector<OutRec> &ord)
-{
-	for (size_t pos = 0; pos < b.size(); pos++) {
-		if (p.vm_runstart) {
-			if (!p.run_class.has(b[pos]) || (pos > 0 && p.run_class.has(b[pos - 1]))) continue;
-			size_t k = 0;
-			while (pos + k < b.size() && p.run_class.has(b[pos + k])) k++;
-			if (k >= (size_t)p.run_min) ord.push_back(OutRec{unit, (uint32_t)pos, 0, 0});
-		} else {
-			for (auto &q : p.seqs)
-				if (seq_at(q, b.data(), b.size(), pos)) { ord.push_back(OutRec{unit, (uint32_t)pos, (uint32_t)q.size(), 0}); break; }
-		}
-	}
-}
-
-static void exclusive(uint32_t *v, size_t n, uint32_t *total)
-{
-	uint32_t acc = 0;
-	for (size_t i = 0; i < n; i++) { const uint32_t f = v[i]; v[i] = acc; acc += f; }
-	if (total) *total = acc;
-}
-
-enum Path { P_TWO, P_DENSE_TWO, P_RUN };
+enum { P_TWO, P_DENSE_TWO, P_RUN };
 static const char *path_name[3] = {"two-outcome", "dense two-outcome", "class-repeat chain"};
 
-// launch_resolve_count + launch_resolve_write of resolve_kernels.cu for one batch, on the host (the device's block scans are
-// plain prefix sums here).  0 ok, -1 VM limit
-static int run_path(const Program &p, const std::vector<const Bytes *> &subj, uint32_t mode, Path path, std::vector<std::vector<M>> &out)
+// the batch through the shipped launch sequence on the path the planner picks with the chain paths forced on (what
+// GSCAN_CHAIN=1 selects), the unit budgets clamped to kModelSteps.  0 ok, -1 VM limit
+static int run_path(const Program &p, const std::vector<const Bytes *> &subj, uint32_t mode, std::vector<std::vector<M>> &out)
 {
-	const uint32_t nu = (uint32_t)subj.size();
-	std::vector<DevUnit> du(nu);
-	for (uint32_t u = 0; u < nu; u++) {
-		memset(&du[u], 0, sizeof du[u]);
-		du[u].ptr = (uint64_t)(uintptr_t)subj[u]->data();
-		du[u].len = (uint32_t)subj[u]->size();
-		du[u].base_off = 1000u * u;
-		du[u].file_id = 7 + u;
-	}
-	ResolveArgs R;
-	memset(&R, 0, sizeof R);
-	uint32_t tot[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-	std::vector<unsigned long long> vbud(nu);
-	std::vector<uint32_t> us(nu + 1, 0u), vus(nu + 1, 0u), uo(nu + 1, 0u), flag, buf;
-	std::vector<OutRec> ord, ordb, vord;
-	std::vector<TileDesc> tds;
-	R.units = du.data(); R.n_units = nu; R.totals = tot; R.vm_limit = tot + 2; R.vm_budget = vbud.data();
-	R.unit_out = uo.data(); R.mode = mode; R.minlen = (uint32_t)p.minlen; R.engine = GSCAN_ENGINE_VM; R.run_min = (uint32_t)p.run_min;
-	for (int i = 0; i < 8; i++) R.bitmap[i] = path == P_DENSE_TWO ? p.first_set.w[i] : p.run_class.w[i];
-	R.vm_code = p.vm_code.data(); R.vm_sets = p.vm_sets.data();
-	R.vm_par = 1; R.vm_two = path != P_RUN; R.vm_chain_run = path == P_RUN;
-	auto each = [&](uint32_t n, auto fn) { for (uint32_t i = 0; i < n; i++) { model_threadIdx.x = i; fn(); } model_threadIdx.x = 0; };
-	out.assign(nu, std::vector<M>());
-	uint32_t cap = 0, levels = 2;
-	if (path != P_DENSE_TWO) {
-		for (uint32_t u = 0; u < nu; u++) { candidates(p, *subj[u], u, ord); us[u + 1] = (uint32_t)ord.size(); }
-		const uint32_t nc = (uint32_t)ord.size();
-		if (nc == 0) return 0;
-		cap = R.vm_two ? 2 * nc : nc;
-		while ((1u << levels) < cap) levels++;
-		buf.assign((size_t)(levels + 4) * cap, 0u); flag.assign(cap, 0u); vord.assign(cap, OutRec{0, 0, 0, 0}); ordb.assign(nc, OutRec{0, 0, 0, 0});
-		R.ord = ord.data(); R.unit_start = us.data(); R.total_cand = nc;
-		R.chain = 1; R.chain_levels = levels; R.chain_cap = cap; R.chain_buf = buf.data();
-		R.vm_ord = vord.data(); R.vm_flag = flag.data(); R.vm_unit_start = vus.data(); R.vm_ord_b = ordb.data();
-		tot[0] = nc;
-		each(nu, [&] { k_vm_budget_init(R); });
-		for (auto &v : vbud) v = std::min(v, kModelSteps);
-		each(nc, [&] { k_vm_attempts(R); });
-		exclusive(flag.data(), cap, &tot[4]);
-		each(nc, [&] { k_vm_compact(R); });
-		each(nu + 1, [&] { k_vm_unit_starts(R); });
-	} else {
-		// tiles of 256 bytes (the device's are 4 .. 64 KiB; the block -> tile -> unit arithmetic is the same)
-		const uint32_t tshift = 8;
-		for (uint32_t u = 0; u < nu; u++) {
-			du[u].first_tile = (uint32_t)tds.size();
-			const size_t len = subj[u]->size();
-			for (size_t off = 0; off < len; off += (size_t)1 << tshift) {
-				TileDesc t;
-				memset(&t, 0, sizeof t);
-				t.src = du[u].ptr + off; t.unit = u; t.off = (uint32_t)off;
-				t.len = (uint32_t)std::min<size_t>((size_t)1 << tshift, len - off); t.ulen = (uint32_t)len;
-				tds.push_back(t);
-			}
-		}
-		const uint32_t blocks = (uint32_t)tds.size() << (tshift - 6);
-		flag.assign(blocks + 1, 0u);
-		R.tiles = tds.data(); R.dense_tile_shift = tshift; R.dense_blocks = blocks; R.vm_flag = flag.data(); R.vm_unit_start = vus.data();
-		each(nu, [&] { k_vm_budget_init(R); });
-		for (auto &v : vbud) v = std::min(v, kModelSteps);
-		each(blocks, [&] { k_vm_dense<false>(R); });
-		if (tot[2]) return -1;
-		exclusive(flag.data(), blocks, &tot[4]);
-		cap = tot[4];
-		if (cap == 0) return 0;
-		while ((1u << levels) < cap) levels++;
-		buf.assign((size_t)(levels + 4) * cap, 0u); vord.assign(cap, OutRec{0, 0, 0, 0});
-		R.vm_ord = vord.data();
-		R.chain = 1; R.chain_levels = levels; R.chain_cap = cap; R.chain_buf = buf.data();
-		each(nu, [&] { k_vm_budget_init(R); });
-		for (auto &v : vbud) v = std::min(v, kModelSteps);
-		each(blocks, [&] { k_vm_dense<true>(R); });
-		each(nu + 1, [&] { k_vm_dense_unit_starts(R); });
-		R.vm_ready = 1; R.total_cand = cap;
-	}
-	if (tot[2]) return -1;
-	ResolveArgs C = R;
-	C.ord = R.vm_ord; C.unit_start = R.vm_unit_start; C.totals = R.totals + 4; // chain_view()
-	const uint32_t nodes = tot[4];
-	uint32_t *mark = buf.data() + (size_t)levels * cap, *rank = mark + cap;
-	if (R.vm_two) {
-		exclusive(buf.data() + (size_t)(levels + 2) * cap, cap, &tot[5]);
-		each(nodes, [&] { k_two_blist(C); });
-	}
-	const bool follow = mode != GSCAN_MODE_FIRST;
-	if (follow) {
-		if (R.vm_chain_run) each(nodes, [&] { k_vm_resume(C); });
-		each(nodes, [&] { k_chain_next(C); });
-		for (uint32_t k = 1; k < levels; k++) each(nodes, [&] { k_chain_double(C, k); });
-	}
-	each(nu, [&] { k_chain_heads(C); });
-	if (follow) for (uint32_t k = levels; k-- > 0;) each(nodes, [&] { k_chain_spread(C, k); });
-	each(nodes, [&] { k_chain_unmark(C); });
-	if (R.vm_chain_run) {
-		each(nodes, [&] { k_chain_entry_init(C); });
-		if (follow) each(nodes, [&] { k_chain_entry(C); });
-	}
-	if (tot[2]) return -1;
-	std::copy(mark, mark + cap, rank);
-	exclusive(rank, cap, nullptr);
-	each(nu, [&] { k_chain_count(C); });
-	std::vector<uint32_t> cnt(uo.begin(), uo.begin() + nu);
-	uint32_t total = 0;
-	exclusive(uo.data(), nu, &total);
-	std::vector<FinalRec> fin(total + 1);
-	C.out = fin.data();
-	C.total_cand = cap;
-	each(cap, [&] { k_chain_write(C); });
-	for (uint32_t u = 0; u < nu; u++)
-		for (uint32_t k = 0; k < cnt[u]; k++) {
-			const FinalRec &r = fin[uo[u] + k];
-			if (r.file_id != du[u].file_id) return -2;
-			out[u].push_back(M{r.start - du[u].base_off, r.len});
-		}
-	return 0;
+	ModelBatch b(p, subj);
+	HostExec x;
+	x.after_budget_init = [](const ResolveArgs &R) { for (uint32_t u = 0; u < R.n_units; u++) R.vm_budget[u] = std::min(R.vm_budget[u], kModelSteps); };
+	return b.run(p, mode, b.plan(p, mode, CHAIN_ON), x, out);
 }
 
 static bool same(const std::vector<M> &g, const go_matches &w)
@@ -318,18 +147,17 @@ int main(int argc, char **argv)
 					if (reach_violations(p, subjects, p.vm_reach - 1) > 0) n_caught++;
 				}
 			}
-			Path path;
-			if (p.vm_runstart) {
-				if (p.vm_reach != 0 || p.vm_lead == VM_Q_LAZY) continue;
-				path = P_RUN;
-			} else if (p.vm_reach == 1) path = p.vm_dense ? P_DENSE_TWO : P_TWO;
-			else continue;
+			// the paths of this check (reach 0 without a leading class repeat: model_check.cc); a batch with no candidates plans NONE
+			const uint32_t planned = plan_resolve(p, GSCAN_MODE_ALL, 1, 1, 1, 1, CHAIN_ON);
+			const int path = planned == GSCAN_RESOLVE_VM_TWO ? P_TWO : planned == GSCAN_RESOLVE_VM_DENSE_TWO ? P_DENSE_TWO
+			               : planned == GSCAN_RESOLVE_VM_RUN_CHAIN ? P_RUN : -1;
+			if (path < 0) continue;
 			for (int m = 0; m < 3; m++) {
 				for (size_t k = 0; k < all.size(); k++) {
 					go_matches w = {0, 0, 0};
 					if (go_scan_window(re, all[k].data(), all[k].size(), 0, 0, modes[m], strict, &w) != 0) { go_matches_free(&w); n_limit++; continue; }
 					std::vector<std::vector<M>> got;
-					const int rc = run_path(p, {&all[k]}, dmodes[m], path, got);
+					const int rc = run_path(p, {&all[k]}, dmodes[m], got);
 					if (rc == -1) { n_limit++; go_matches_free(&w); continue; }
 					if (rc != 0 || !same(got[0], w)) {
 						bad++;
@@ -347,7 +175,7 @@ int main(int argc, char **argv)
 					const bool ok0 = go_scan_window(re, all[k].data(), all[k].size(), 0, 0, modes[m], strict, &w[0]) == 0;
 					const bool ok1 = go_scan_window(re, all[k + 1].data(), all[k + 1].size(), 0, 0, modes[m], strict, &w[1]) == 0;
 					std::vector<std::vector<M>> got;
-					const int rc = ok0 && ok1 ? run_path(p, {&all[k], &all[k + 1]}, dmodes[m], path, got) : -1;
+					const int rc = ok0 && ok1 ? run_path(p, {&all[k], &all[k + 1]}, dmodes[m], got) : -1;
 					if (rc == -1) n_limit++;
 					else if (rc != 0 || !same(got[0], w[0]) || !same(got[1], w[1])) {
 						bad++;

@@ -1,6 +1,7 @@
 """What the pattern compiler hands to the device, interpreted on the CPU and compared with the oracle (no GPU):
 tests/model_check.cc runs the compiled Program the way the resolve kernels do -- with the device VM's own source,
-extracted verbatim from grab_b200/csrc/resolve_kernels.cu and compiled for the host -- inside the reference's loop."""
+extracted verbatim from grab_b200/csrc/resolve_kernels.cu and compiled for the host -- inside the reference's loop, and
+every resolve path through the launch sequence the device runs (tests/model_host.h)."""
 import os
 import subprocess
 
@@ -13,7 +14,7 @@ BEGIN = "// ---- device backtracking VM (general patterns) ----"
 END = "// ---- 4. generic u32 block sums / exclusive scan (per-unit match counts -> output slots) ----"
 
 
-def test_compiled_programs_match_the_oracle(tmp_path):
+def test_compiled_programs_and_the_launch_sequence_match_the_oracle(tmp_path):
     src = open(os.path.join(ROOT, "grab_b200", "csrc", "resolve_kernels.cu")).read()
     assert BEGIN in src and END in src
     snippet = src[src.index(BEGIN):src.index(END)]

@@ -32,7 +32,7 @@ HAND = [
 ]
 
 
-def test_start_sensitive_paths_match_the_oracle(tmp_path):
+def test_start_sensitive_paths_through_the_launch_sequence_match_the_oracle(tmp_path):
     src = open(os.path.join(ROOT, "grab_b200", "csrc", "resolve_kernels.cu")).read()
     assert BEGIN in src and END in src
     snippet = src[src.index(BEGIN):src.index(END)]
