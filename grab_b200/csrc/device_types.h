@@ -24,25 +24,13 @@ struct Geom {
 };
 typedef Geom<16, 3, 4096> GeomStream;  // memory-bound: the FIXED filters
 // RUN (class runs): ALU/issue-bound, 24 warps; 4 KiB slices with a 2-deep ring do half the ring work per byte of
-// <24, 4, 2048>.  GS_BAL_* : tuning override (make NAME=x DEFS=-DGS_BAL_W=...)
-#ifndef GS_BAL_W
-#define GS_BAL_W 24
-#define GS_BAL_R 2
-#define GS_BAL_S 4096
-#endif
-typedef Geom<GS_BAL_W, GS_BAL_R, GS_BAL_S> GeomBalanced;
+// <24, 4, 2048>
+typedef Geom<24, 2, 4096> GeomBalanced;
 // hashed engine: issue-bound, wants warps (20 = 5 per scheduler) and
 // long slices (fewer ring refills per byte): 2 x 4 KiB per warp, which leaves 32 KiB for the table
-#ifndef GS_HASH_W
-#define GS_HASH_W 20
-#endif
-typedef Geom<GS_HASH_W, 2, 4096> GeomHash;
+typedef Geom<20, 2, 4096> GeomHash;
 // balanced pair filter (FixedBEngine): issue-bound like the hashed engine
-#ifndef GS_PAIR_W
-#define GS_PAIR_W 20
-#define GS_PAIR_R 2
-#endif
-typedef Geom<GS_PAIR_W, GS_PAIR_R, 4096> GeomPair;
+typedef Geom<20, 2, 4096> GeomPair;
 
 struct ScanGeom { int warps, ring, slice; }; // host-side mirror of the chosen Geom
 
@@ -81,13 +69,14 @@ struct FixedParams {
 	const uint32_t *seq_off;  // [nseq] index into seq_pos
 	const uint32_t *seq_pos;  // per position: mask | val << 8 | cls << 16 (cls 0xffff: none)
 	const uint32_t *cls_bm;   // [ncls][8] bitmaps for positions that are not a masked equality
-	// triples (anchor, anchor + delta, anchor + d2): stage 2 of the pair filter (flagged rows only), or --
-	// stage1_triples -- the stage-1 filter itself (Fixed3Engine; sh1/sh2 = 8*delta, 8*d2 funnel-shift amounts)
-	uint32_t n2, d2, stage1_triples, exact3, sh1, sh2;
-	// balanced pair filter (FixedBEngine): test k in subtract form (w | 0x80..) + b_c0[k] / XOR form ^ b_x0[k]; the third byte
-	// of alternative k (stage 2, aligned with test k) is ((s2 & b_m2[k]) ^ b_v2[k]) == 0, s2 = the bytes b_sh2 / 8 further on
-	uint32_t b_engine, b_aligned, b_sh2;
-	uint32_t b_c0[8], b_c1[8], b_x0[8], b_x1[8], b_m2[8], b_v2[8];
+	// triples (anchor, anchor + delta, anchor + d2): stage 2 of the pair filter (flagged rows only), or the stage-1
+	// filter itself (Fixed3Engine; sh1/sh2 = 8*delta, 8*d2 funnel-shift amounts, 8-byte aligned: the triple filter reads
+	// them with one 64-bit load)
+	uint32_t n2, d2, sh1, sh2, exact3;
+	// balanced pair filter (FixedBEngine): test k is (w | 0x80..) + b_c0[k]; the third byte of alternative k (stage 2,
+	// aligned with test k) is ((s2 & b_m2[k]) ^ b_v2[k]) == 0, s2 = the bytes b_sh2 / 8 further on
+	uint32_t b_aligned, b_sh2;
+	uint32_t b_c0[8], b_c1[8], b_m2[8], b_v2[8];
 	uint32_t t2_m0[16], t2_v0[16], t2_m1[16], t2_v1[16], t2_m2[16], t2_v2[16];
 };
 
@@ -98,7 +87,6 @@ struct HashParams {
 	uint32_t nslots;     //   slot = umulhi(h, nslots): IMADs only, nothing on the ALU pipe
 	uint32_t stride;     // bytes between slots in shared memory: 128 when the table is replicated per bank, else 4
 	uint32_t neg1;       // == 0xffffffff, opaque to the compiler: h * neg1 + entry is an IMAD (FMA pipe) where a XOR would be ALU
-	uint32_t pow2_shift, pow2_mask; // power-of-two replicated table: row offset = (h >> pow2_shift) & pow2_mask (0: not a power of two)
 	// class prefilter (sparse path): every key byte lies in [pre_lo, pre_hi] (one range inside 0x01-0x7d); a position can
 	// only hold a key when its hash_len bytes all pass x in [pre_lo, pre_hi + 1] -- tested SWAR, the table is then probed
 	// at the surviving positions only.  pre_enable == 0: no usable range, every position is probed (dense path).
@@ -114,7 +102,6 @@ struct HashParams {
 	const uint32_t *slot_first; // [nslots] first index into slot_seqs
 	const uint32_t *slot_count; // [nslots]
 	const uint32_t *slot_seqs;  // alternatives of a key, preference order
-	uint32_t uniform_len, maxlen;
 	const uint16_t *seq_len;
 	const uint32_t *seq_off;
 	const uint32_t *seq_pos;
@@ -126,10 +113,7 @@ constexpr int kHashMaxSlots = 8192;
 // 16 lookups per 512-byte row that alone caps the kernel's throughput).  512 slots x 128 bytes = 64 KiB, beside a 20-warp ring
 // of 2 x 4 KiB slots
 constexpr uint32_t kHashReplicatedSlots = 512;
-#ifndef GS_HASH_COPIES
-#define GS_HASH_COPIES 32
-#endif
-static inline uint32_t hash_table_copies(uint32_t nslots) { return nslots <= kHashReplicatedSlots ? (uint32_t)GS_HASH_COPIES : 1u; }
+static inline uint32_t hash_table_copies(uint32_t nslots) { return nslots <= kHashReplicatedSlots ? 32u : 1u; }
 
 struct RunParams {
 	uint32_t one;         // == 1, opaque (see FixedParams)

@@ -33,6 +33,7 @@ using namespace gscan;
 // ------------------------------------------------------------------------------------------
 struct gscan_pattern {
 	Program prog;
+	int32_t kernel; // GSCAN_KERNEL_*: the scan kernel that serves the pattern (scan_kernel_for)
 	// host images of the device tables (FIXED engine)
 	std::vector<uint16_t> seq_len;
 	std::vector<uint32_t> seq_off, seq_pos, cls_bm;
@@ -160,6 +161,26 @@ static inline uint32_t round16(uint32_t x) { return (x + 15u) & ~15u; }
 // ------------------------------------------------------------------------------------------
 // pattern
 // ------------------------------------------------------------------------------------------
+// The scan kernel (GSCAN_KERNEL_*) that serves a compiled program, F: the filter gscan_compile built for it.  The only place
+// this is decided; the rules are tried in order.
+static int32_t scan_kernel_for(const Program &pr, const FixedParams &F)
+{
+	// no candidate filter: the VM walk tries the positions itself
+	if (pr.kind == ENGINE_NONE || pr.vm_dense) return GSCAN_KERNEL_NONE;
+	if (pr.kind == ENGINE_RUN) return GSCAN_KERNEL_RUN;
+	if (pr.use_hash) return GSCAN_KERNEL_HASH;
+	// balanced pair filter: 2..8 exact byte pairs, when its stage 2 tests one third byte per pair test or the pairs alone
+	// rarely flag a row
+	const size_t nt = pr.tests.size();
+	if (F.exact && nt >= 2 && nt <= 8 && pr.delta >= 1 && pr.delta <= 4 && (F.b_aligned || pr.pair_flag_prior * 512.0 <= 0.01))
+		return GSCAN_KERNEL_BALANCED;
+	// a 4 KiB slice has 8 rows of 512 bytes; once more than a few percent of the rows get flagged the slow path
+	// dominates, and three filter bytes (+2 ops per word) are cheaper than visiting it
+	if (!pr.triples.empty() && pr.triples.size() <= 8 && pr.delta >= 1 && pr.delta <= 3 && pr.pair_flag_prior * 512.0 > 0.01)
+		return GSCAN_KERNEL_TRIPLE;
+	return GSCAN_KERNEL_PAIR;
+}
+
 extern "C" int gscan_compile(const char *pattern, size_t len, uint32_t flags, gscan_pattern **out)
 {
 	if (!pattern || !out) { g_last_error = "gscan_compile: null argument"; return -1; }
@@ -185,7 +206,6 @@ extern "C" int gscan_compile(const char *pattern, size_t len, uint32_t flags, gs
 		if (!pr.delta) F.exact = 0; // single-byte filter: the second term must vanish through its zero mask
 		F.n2 = (uint32_t)pr.triples.size();
 		F.d2 = (uint32_t)pr.delta2;
-		F.stage1_triples = pr.stage1_triples ? 1u : 0u;
 		F.sh1 = 8u * (uint32_t)pr.delta;
 		F.sh2 = 8u * (uint32_t)pr.delta2;
 		F.exact3 = 1;
@@ -203,15 +223,14 @@ extern "C" int gscan_compile(const char *pattern, size_t len, uint32_t flags, gs
 			F.m0[k] = rep4(pr.tests[k].m0); F.v0[k] = rep4(pr.tests[k].v0);
 			F.m1[k] = rep4(pr.tests[k].m1); F.v1[k] = rep4(pr.tests[k].v1);
 		}
-		{ // balanced pair filter (FixedBEngine): exact byte pairs, 2..8 tests; stage 2 needs one third-byte test per pair test
-			F.b_engine = 0; F.b_aligned = 0; F.b_sh2 = 8u * (uint32_t)pr.delta2;
-			for (int k = 0; k < 8; k++) { F.b_c0[k] = 0; F.b_c1[k] = 0; F.b_x0[k] = 0; F.b_x1[k] = 0; F.b_m2[k] = 0; F.b_v2[k] = 0xffffffffu; }
+		{ // balanced pair filter (FixedBEngine): exact byte pairs; stage 2 needs one third-byte test per pair test
+			F.b_aligned = 0; F.b_sh2 = 8u * (uint32_t)pr.delta2;
+			for (int k = 0; k < 8; k++) { F.b_c0[k] = 0; F.b_c1[k] = 0; F.b_m2[k] = 0; F.b_v2[k] = 0xffffffffu; }
 			const size_t nt = pr.tests.size();
 			bool aligned = !pr.triples.empty() && pr.triples.size() == nt;
 			for (size_t k = 0; k < nt && k < 8; k++) {
 				const FilterTest &t = pr.tests[k];
 				F.b_c0[k] = 0u - rep4(t.v0 & 0x7f); F.b_c1[k] = 0u - rep4(t.v1 & 0x7f);
-				F.b_x0[k] = rep4(t.v0 | 0x80); F.b_x1[k] = rep4(t.v1 | 0x80);
 				int hit = -1, hits = 0;
 				for (size_t j = 0; j < pr.triples.size(); j++) {
 					const Program::Triple &q = pr.triples[j];
@@ -221,10 +240,6 @@ extern "C" int gscan_compile(const char *pattern, size_t len, uint32_t flags, gs
 				else { F.b_m2[k] = rep4(pr.triples[(size_t)hit].m2); F.b_v2[k] = rep4(pr.triples[(size_t)hit].v2); }
 			}
 			F.b_aligned = aligned ? 1u : 0u;
-			const char *off = getenv("GSCAN_NO_FIXEDB"); // A/B switch for measurements
-			if (F.exact && nt >= 2 && nt <= 8 && pr.delta >= 1 && pr.delta <= 4 && !pr.use_hash && !(off && *off == '1') &&
-			    (aligned || pr.pair_flag_prior * 512.0 <= 0.01))
-				F.b_engine = 1;
 		}
 		F.anchor = (uint32_t)pr.anchor;
 		F.nseq = (uint32_t)pr.seqs.size();
@@ -262,15 +277,6 @@ extern "C" int gscan_compile(const char *pattern, size_t len, uint32_t flags, gs
 			H.nslots = pr.hash_slots;
 			H.stride = hash_table_copies(pr.hash_slots) * 4u;
 			H.neg1 = 0xffffffffu;
-			H.pow2_shift = H.pow2_mask = 0;
-			if (H.stride == 128u && (H.nslots & (H.nslots - 1u)) == 0u && H.nslots >= 2u) {
-				uint32_t lg = 0;
-				while ((1u << lg) < H.nslots) lg++;
-				H.pow2_shift = 32u - lg - 7u;          // slot = h >> (32 - lg); row offset = slot * 128
-				H.pow2_mask = (H.nslots - 1u) << 7;
-			}
-			H.uniform_len = F.uniform_len;
-			H.maxlen = F.maxlen;
 			// class prefilter of the sparse path: one byte range that holds every key byte
 			H.one = 1;
 			H.hash_len = (uint32_t)pr.hash_len;
@@ -329,6 +335,7 @@ extern "C" int gscan_compile(const char *pattern, size_t len, uint32_t flags, gs
 		}
 		for (int i = 0; i < 8; i++) R.bitmap[i] = pr.run_class.w[i];
 	}
+	p->kernel = scan_kernel_for(pr, p->fixed);
 	*out = p;
 	return 0;
 }
@@ -350,11 +357,7 @@ extern "C" int gscan_pattern_get_info(const gscan_pattern *p, gscan_pattern_info
 	o->filter_anchor = p->prog.anchor;
 	o->filter_delta = p->prog.delta;
 	o->reserved = 0;
-	if (p->prog.kind == ENGINE_NONE || (p->prog.use_vm && p->prog.vm_dense)) o->scan_kernel = GSCAN_KERNEL_NONE;
-	else if (p->prog.kind == ENGINE_RUN) o->scan_kernel = GSCAN_KERNEL_RUN;
-	else if (p->prog.use_hash) o->scan_kernel = GSCAN_KERNEL_HASH;
-	else if (p->fixed.b_engine) o->scan_kernel = GSCAN_KERNEL_BALANCED;
-	else o->scan_kernel = p->fixed.stage1_triples ? GSCAN_KERNEL_TRIPLE : GSCAN_KERNEL_PAIR;
+	o->scan_kernel = p->kernel;
 	return 0;
 }
 
@@ -826,10 +829,8 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 	}
 	if (ensure_pattern(ctx, pat) < 0) return -1;
 
-	const bool hashed = pat->prog.kind == ENGINE_FIXED && pat->prog.use_hash;
-	const uint32_t table_bytes = hashed ? pat->prog.hash_slots * 4u * hash_table_copies(pat->prog.hash_slots) : 0u;
-	const bool fixedb = pat->prog.kind == ENGINE_FIXED && !hashed && pat->fixed.b_engine;
-	const ScanGeom geom = scan_geom(hashed ? 4 : (fixedb ? 5 : (int)pat->prog.kind), pat->prog.kind == ENGINE_FIXED ? (uint32_t)pat->prog.tests.size() : 99u);
+	const uint32_t table_bytes = pat->kernel == GSCAN_KERNEL_HASH ? pat->prog.hash_slots * 4u * hash_table_copies(pat->prog.hash_slots) : 0u;
+	const ScanGeom geom = scan_geom(pat->kernel);
 	uint32_t spt_shift = b->tile_shift;
 	for (int sl = geom.slice; sl > 1; sl >>= 1) spt_shift--; // log2(tile bytes / slice bytes)
 	const uint32_t n_segs = b->n_tiles << spt_shift;
@@ -871,9 +872,7 @@ extern "C" int gscan_batch_scan(gscan_ctx *ctx, const gscan_pattern *pat, gscan_
 		A.chunk = (uint32_t)std::min<size_t>(std::max<size_t>(A.cand_cap / ((size_t)8 * (size_t)grid * (size_t)geom.warps), 32), 1024);
 		CK(ctx, launch_fill_u32(reinterpret_cast<uint32_t *>(ctx->cursor.p), 12, 0u, ctx->stream));
 		CK(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
-		if (hashed) CK(ctx, launch_scan_hash(A, ctx->pat_hash, grid, ctx->stream));
-		else if (pat->prog.kind == ENGINE_FIXED) CK(ctx, launch_scan_fixed(A, ctx->pat_fixed, pat->prog.delta, geom, grid, ctx->stream));
-		else CK(ctx, launch_scan_run(A, pat->run, geom, grid, ctx->stream));
+		CK(ctx, launch_scan(pat->kernel, A, ctx->pat_fixed, ctx->pat_hash, pat->run, pat->prog.delta, grid, ctx->stream));
 		CK(ctx, cudaEventRecord(ctx->ev[1], ctx->stream));
 		CK(ctx, cudaMemcpyAsync(h_cursor, ctx->cursor.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
 		CK(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1159,8 +1158,7 @@ extern "C" int gscan_tma_probe(gscan_ctx *ctx, gscan_batch *b, int geom, float *
 {
 	if (!ctx || !b || !b->n_tiles) return fail(ctx, "gscan_tma_probe: null argument");
 	CK(ctx, cudaSetDevice(ctx->device));
-	const ScanGeom g = geom == 0 ? ScanGeom{GeomStream::kWarps, GeomStream::kRing, GeomStream::kSlice}
-	                             : ScanGeom{GeomBalanced::kWarps, GeomBalanced::kRing, GeomBalanced::kSlice};
+	const ScanGeom g = scan_geom(geom == 0 ? GSCAN_KERNEL_PAIR : GSCAN_KERNEL_RUN);
 	uint32_t spt_shift = b->tile_shift;
 	for (int sl = g.slice; sl > 1; sl >>= 1) spt_shift--;
 	const uint32_t n_segs = b->n_tiles << spt_shift;

@@ -10,11 +10,14 @@
 namespace gscan {
 
 size_t scan_smem_bytes(const ScanGeom &g, bool look_behind);
-ScanGeom scan_geom(int engine, uint32_t n_tests_or_ranges);
-cudaError_t launch_scan_fixed(const ScanArgs &A, const FixedParams &P, int delta, const ScanGeom &g, int grid, cudaStream_t st);
-cudaError_t launch_scan_hash(const ScanArgs &A, const HashParams &P, int grid, cudaStream_t st);
+// kernel: the pattern's GSCAN_KERNEL_* value (include/gscan.h), picked once when the pattern is compiled
+ScanGeom scan_geom(int kernel);
+// the scan kernel instantiation for `kernel` and the pattern's filter: F (PAIR, TRIPLE, BALANCED; delta: its filter
+// distance), H (HASH) or R (RUN); the other two are not read.  NONE is an error.
+cudaError_t launch_scan(int kernel, const ScanArgs &A, const FixedParams &F, const HashParams &H, const RunParams &R, int delta,
+                        int grid, cudaStream_t st);
+// gscan_tma_probe: the null engine on geometry 0 (scan_geom(GSCAN_KERNEL_PAIR)) or 1 (scan_geom(GSCAN_KERNEL_RUN))
 cudaError_t launch_scan_null(const ScanArgs &A, int geom, int grid, cudaStream_t st);
-cudaError_t launch_scan_run(const ScanArgs &A, const RunParams &P, const ScanGeom &g, int grid, cudaStream_t st);
 
 struct DevUnit {
 	uint64_t ptr;        // device address of the unit's bytes

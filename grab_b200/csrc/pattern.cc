@@ -1331,10 +1331,7 @@ bool compile_pattern(const char *pat, size_t len, uint32_t flags, Program &out, 
 		out.triples.clear();
 		return true;
 	}
-	// a 4 KiB slice has 8 rows of 512 bytes; once more than a few percent of the rows get flagged the slow path
-	// dominates, and three filter bytes (+2 ops per word) are cheaper than visiting it
 	out.pair_flag_prior = best_p;
-	out.stage1_triples = !out.triples.empty() && out.triples.size() <= 8 && out.delta >= 1 && out.delta <= 3 && best_p * 512.0 > 0.01;
 
 	// ---- can two matches overlap?  If not, the greedy resolve keeps every candidate ----
 	bool disjoint = true;

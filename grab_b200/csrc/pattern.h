@@ -79,7 +79,6 @@ struct Program {
 	struct Triple { uint8_t m0, v0, m1, v1, m2, v2; };
 	std::vector<Triple> triples;      // stage-2 refinement with a third byte at anchor+delta2 (empty: none)
 	int delta2 = 0;
-	bool stage1_triples = false;      // the pair filter would flag too many rows: filter on the triples right away
 	double pair_flag_prior = 0;       // estimated probability that the pair filter flags a byte (static text prior)
 	bool disjoint = false;            // no two matches can ever overlap => resolve is a pure copy
 

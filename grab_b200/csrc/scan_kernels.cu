@@ -30,10 +30,6 @@
 #include "swar.h"
 #include "kernels.h"
 
-#ifndef GS_RUN_STREAM
-#define GS_RUN_STREAM 0
-#endif
-
 namespace gscan {
 
 // ------------------------------------------------------------------------------------------
@@ -431,36 +427,27 @@ struct Fixed3Engine {
 //     with V = the pattern byte & 0x7f replicated: no byte borrows (0x80+x - v >= 1) and a byte of a is 0x80 iff
 //     the text byte equals the pattern byte (mod bit 7: a superset, the verification is exact).  One LOP3 then
 //     forms t = (a | b) ^ 0x80808080 -- zero byte iff both match -- and the usual zero-byte test (IMAD + LOP3)
-//     ORs it into the row's flag word: 2 ALU-pipe + 3 FMA-pipe instructions per test and word instead of 3 + 1
-//     (GS_FB_A of the K tests can be switched back to the XOR form to balance the two pipes);
+//     ORs it into the row's flag word: 2 ALU-pipe + 3 FMA-pipe instructions per test and word instead of 3 + 1;
 //   * the cheap pair test flags one row in six on random text, so the third byte is NOT tested up front but in an
 //     inline stage 2 on the flagged rows only, reusing the kept t words (t | third-byte mismatch), and only rows
 //     that survive both stages visit the out-of-line verification.
 // ------------------------------------------------------------------------------------------
-#ifndef GS_FB_A
-#define GS_FB_A 0
-#endif
 template <int D, int K, bool ALIGNED>
 struct FixedBEngine {
 	typedef FixedParams Params;
 	static constexpr bool kLookBehind = false, kLookAhead = true, kMergeCopies = true;
-	static constexpr int kA = GS_FB_A < K ? GS_FB_A : K; // tests [0, kA) in XOR form, [kA, K) in subtract form
 	static __device__ __forceinline__ void prologue(const FixedParams &, uint8_t *) {}
 
 	// t words of one text word: zero byte <=> pair test k passes at that byte (bit 7 of the text ignored).  Bit 7 of every
-	// byte of t is clear by construction (XOR form: both operands have it set; subtract form: a | b is never 0x00, so
-	// masking bit 7 leaves a zero byte exactly where a == b == 0x80), which halves the zero-byte test: t - 0x01 sets
-	// bit 7 where t is zero (or above a zero byte: a superset), no "& ~t" needed.
+	// byte of t is clear by construction (a | b is never 0x00, so masking bit 7 leaves a zero byte exactly where
+	// a == b == 0x80), which halves the zero-byte test: t - 0x01 sets bit 7 where t is zero (or above a zero byte: a
+	// superset), no "& ~t" needed.
 	static __device__ __forceinline__ void word_t(const FixedParams &P, uint32_t w80, uint32_t s80, uint32_t (&t)[K])
 	{
 #pragma unroll
 		for (int k = 0; k < K; k++) {
-			if (k < kA) {
-				t[k] = (w80 ^ P.b_x0[k]) | (s80 ^ P.b_x1[k]);
-			} else {
-				const uint32_t a = w80 * P.one + P.b_c0[k], b = s80 * P.one + P.b_c1[k];
-				t[k] = (a | b) & kLow7;
-			}
+			const uint32_t a = w80 * P.one + P.b_c0[k], b = s80 * P.one + P.b_c1[k];
+			t[k] = (a | b) & kLow7;
 		}
 	}
 	static __device__ __forceinline__ uint32_t dec(const FixedParams &P, uint32_t t) { return t * P.one + 0xfefefeffu; }
@@ -527,12 +514,6 @@ struct FixedBEngine {
 // copy the 32 random slots of a warp cost ~3.4 wavefronts and the shared-memory data pipe is the bottleneck (95 %
 // busy, profiles/r01_scan_v5_lits8_single_table_ncu.txt).
 // ------------------------------------------------------------------------------------------
-#ifndef GS_HASH_SUB
-#define GS_HASH_SUB 2
-#endif
-#ifndef GS_HASH_POW2
-#define GS_HASH_POW2 0
-#endif
 struct HashEngine {
 	typedef HashParams Params;
 	static constexpr bool kLookBehind = false, kLookAhead = true, kMergeCopies = true;
@@ -575,23 +556,14 @@ struct HashEngine {
 	// the 32-bit window at byte k of the word pair; the bytes beyond the key fall off the top of window * mulsh
 	static __device__ __forceinline__ uint32_t window(uint32_t lo, uint32_t hi, int k) { return k ? __funnelshift_r(lo, hi, 8 * k) : lo; }
 	static __device__ __forceinline__ uint32_t slot_of(const HashParams &P, uint32_t h) { return __umulhi(h, P.nslots); }
-	// byte offset of the slot's row in the replicated table.  GS_HASH_POW2 (tuning): for a power-of-two table the offset is
-	// a shift and a mask on the ALU pipe instead of IMAD.HI + IMAD on the FMA pipe
-	static __device__ __forceinline__ uint32_t row_of(const HashParams &P, uint32_t h)
-	{
-#if GS_HASH_POW2
-		if (P.pow2_shift) return (h >> P.pow2_shift) & P.pow2_mask;
-#endif
-		return slot_of(P, h) * P.stride;
-	}
 	// tbl: the table in shared memory, for a replicated table already advanced to this lane's bank (+ lane * 4).
 	// Hash, slot and address are three IMADs (FMA pipe); zero <=> the position holds a key of the set.  SUB: the
-	// comparison as entry - h on the FMA pipe instead of entry ^ h on the ALU pipe (GS_HASH_SUB of every 4 positions).
+	// comparison as entry - h on the FMA pipe instead of entry ^ h on the ALU pipe (two of every 4 positions).
 	template <bool SUB>
 	static __device__ __forceinline__ uint32_t probe(const HashParams &P, const uint8_t *tbl, uint32_t y)
 	{
 		const uint32_t h = y * P.mulsh;
-		const uint32_t e = *reinterpret_cast<const uint32_t *>(tbl + row_of(P, h));
+		const uint32_t e = *reinterpret_cast<const uint32_t *>(tbl + slot_of(P, h) * P.stride);
 		return SUB ? h * P.neg1 + e : e ^ h;
 	}
 
@@ -602,10 +574,10 @@ struct HashEngine {
 		uint32_t mn = 0xffffffffu;
 #pragma unroll
 		for (int j = 0; j < 4; j++) {
-			d[4 * j + 0] = probe<(GS_HASH_SUB > 0)>(P, tbl, window(w[j], w[j + 1], 0));
-			d[4 * j + 1] = probe<(GS_HASH_SUB > 1)>(P, tbl, window(w[j], w[j + 1], 1));
-			d[4 * j + 2] = probe<(GS_HASH_SUB > 2)>(P, tbl, window(w[j], w[j + 1], 2));
-			d[4 * j + 3] = probe<(GS_HASH_SUB > 3)>(P, tbl, window(w[j], w[j + 1], 3));
+			d[4 * j + 0] = probe<true>(P, tbl, window(w[j], w[j + 1], 0));
+			d[4 * j + 1] = probe<true>(P, tbl, window(w[j], w[j + 1], 1));
+			d[4 * j + 2] = probe<false>(P, tbl, window(w[j], w[j + 1], 2));
+			d[4 * j + 3] = probe<false>(P, tbl, window(w[j], w[j + 1], 3));
 			mn = __vimin3_u32(mn, d[4 * j + 0], d[4 * j + 1]);
 			mn = __vimin3_u32(mn, d[4 * j + 2], d[4 * j + 3]);
 		}
@@ -682,10 +654,7 @@ struct HashEngine {
 		if (P.hash_len == 3) f &= __funnelshift_r(n1, lop3<0xCA>(0x7fu, n1 >> 1, r8 >> 8), 8);
 		return f;
 	}
-#ifndef GS_HASH_PREMAX
-#define GS_HASH_PREMAX 12
-#endif
-	static constexpr uint32_t kPreMax = GS_HASH_PREMAX; // more flagged positions than this in one lane (of 32): the dense path is cheaper
+	static constexpr uint32_t kPreMax = 12; // more flagged positions than this in one lane (of 32): the dense path is cheaper
 
 	// Rare (a key of the set really is in the block, one 1 KiB block in eight on printable noise): decide the lanes' key
 	// hits and append the matches in position order.  A key hit is first held against the slot's TAIL entry -- what the 8
@@ -1287,11 +1256,13 @@ scan_kernel(const __grid_constant__ ScanArgs A, const __grid_constant__ typename
 // ------------------------------------------------------------------------------------------
 constexpr int kMaxDevices = 64;
 
+template <class G>
+static ScanGeom geom_of() { return ScanGeom{G::kWarps, G::kRing, G::kSlice}; }
+
 template <class Eng, class G>
 static cudaError_t launch_g(const ScanArgs &A, const typename Eng::Params &P, int grid, cudaStream_t st)
 {
-	const ScanGeom g{G::kWarps, G::kRing, G::kSlice};
-	const int smem = (int)(scan_smem_bytes(g, Eng::kLookBehind) + A.extra_smem);
+	const int smem = (int)(scan_smem_bytes(geom_of<G>(), Eng::kLookBehind) + A.extra_smem);
 	// the shared-memory limit is a property of the kernel on a device: raised once per instantiation and device, not per
 	// launch (the largest size asked for so far; the hashed engine's table size varies with the pattern)
 	static std::atomic<int> smem_set[kMaxDevices];
@@ -1307,21 +1278,15 @@ static cudaError_t launch_g(const ScanArgs &A, const typename Eng::Params &P, in
 	return cudaGetLastError();
 }
 
-// Instantiated geometries: the streaming one for single-test filters, the balanced one for everything else.
-template <class Eng, bool STREAM>
-static cudaError_t launch(const ScanArgs &A, const typename Eng::Params &P, const ScanGeom &, int grid, cudaStream_t st)
+// which geometry a kernel (GSCAN_KERNEL_*) runs with: the Geom its case of launch_scan below instantiates
+ScanGeom scan_geom(int kernel)
 {
-	if constexpr (STREAM) return launch_g<Eng, GeomStream>(A, P, grid, st);
-	else return launch_g<Eng, GeomBalanced>(A, P, grid, st);
-}
-
-// which geometry an engine runs with
-ScanGeom scan_geom(int engine, uint32_t n_tests_or_ranges)
-{
-	if (engine == 4 /*FIXED, hashed*/) return ScanGeom{GeomHash::kWarps, GeomHash::kRing, GeomHash::kSlice};
-	if (engine == 5 /*FIXED, balanced pair filter*/) return ScanGeom{GeomPair::kWarps, GeomPair::kRing, GeomPair::kSlice};
-	if (engine == 1 /*FIXED*/ || (engine == 2 && GS_RUN_STREAM)) return ScanGeom{GeomStream::kWarps, GeomStream::kRing, GeomStream::kSlice};
-	return ScanGeom{GeomBalanced::kWarps, GeomBalanced::kRing, GeomBalanced::kSlice};
+	switch (kernel) {
+	case GSCAN_KERNEL_BALANCED: return geom_of<GeomPair>();
+	case GSCAN_KERNEL_HASH: return geom_of<GeomHash>();
+	case GSCAN_KERNEL_RUN: return geom_of<GeomBalanced>();
+	default: return geom_of<GeomStream>(); // PAIR, TRIPLE; NONE runs no scan kernel
+	}
 }
 
 cudaError_t launch_scan_null(const ScanArgs &A, int geom, int grid, cudaStream_t st)
@@ -1331,39 +1296,35 @@ cudaError_t launch_scan_null(const ScanArgs &A, int geom, int grid, cudaStream_t
 	return launch_g<NullEngine, GeomBalanced>(A, P, grid, st);
 }
 
-template <bool EX>
-static cudaError_t launch_fixed3(const ScanArgs &A, const FixedParams &P, const ScanGeom &g, int grid, cudaStream_t st)
+// the per-family K tables of launch_scan: an engine instantiated for K tests runs any count up to K (unused tests never pass)
+template <int D, bool EX>
+static cudaError_t launch_pair(const ScanArgs &A, const FixedParams &P, int grid, cudaStream_t st)
 {
-	switch (P.n2) {
-	case 1: return launch<Fixed3Engine<1, EX>, true>(A, P, g, grid, st);
-	case 2: return launch<Fixed3Engine<2, EX>, true>(A, P, g, grid, st);
-	case 3: return launch<Fixed3Engine<3, EX>, true>(A, P, g, grid, st);
-	case 4: return launch<Fixed3Engine<4, EX>, true>(A, P, g, grid, st);
-	case 5: case 6: return launch<Fixed3Engine<6, EX>, true>(A, P, g, grid, st);
-	default: return launch<Fixed3Engine<8, EX>, true>(A, P, g, grid, st);
+	switch (P.ntests) {
+	case 1: return launch_g<FixedEngine<D, 1, EX>, GeomStream>(A, P, grid, st);
+	case 2: return launch_g<FixedEngine<D, 2, EX>, GeomStream>(A, P, grid, st);
+	case 3: return launch_g<FixedEngine<D, 3, EX>, GeomStream>(A, P, grid, st);
+	case 4: return launch_g<FixedEngine<D, 4, EX>, GeomStream>(A, P, grid, st);
+	case 5: case 6: return launch_g<FixedEngine<D, 6, EX>, GeomStream>(A, P, grid, st);
+	default: return launch_g<FixedEngine<D, 8, EX>, GeomStream>(A, P, grid, st);
 	}
 }
 
-cudaError_t launch_scan_hash(const ScanArgs &A, const HashParams &P, int grid, cudaStream_t st)
+template <bool EX>
+static cudaError_t launch_triple(const ScanArgs &A, const FixedParams &P, int grid, cudaStream_t st)
 {
-	return launch_g<HashEngine, GeomHash>(A, P, grid, st);
-}
-
-template <int D, bool EX>
-static cudaError_t launch_fixed_de(const ScanArgs &A, const FixedParams &P, const ScanGeom &g, int grid, cudaStream_t st)
-{
-	switch (P.ntests) {
-	case 1: return launch<FixedEngine<D, 1, EX>, true>(A, P, g, grid, st);
-	case 2: return launch<FixedEngine<D, 2, EX>, true>(A, P, g, grid, st);
-	case 3: return launch<FixedEngine<D, 3, EX>, true>(A, P, g, grid, st);
-	case 4: return launch<FixedEngine<D, 4, EX>, true>(A, P, g, grid, st);
-	case 5: case 6: return launch<FixedEngine<D, 6, EX>, true>(A, P, g, grid, st);
-	default: return launch<FixedEngine<D, 8, EX>, true>(A, P, g, grid, st);
+	switch (P.n2) {
+	case 1: return launch_g<Fixed3Engine<1, EX>, GeomStream>(A, P, grid, st);
+	case 2: return launch_g<Fixed3Engine<2, EX>, GeomStream>(A, P, grid, st);
+	case 3: return launch_g<Fixed3Engine<3, EX>, GeomStream>(A, P, grid, st);
+	case 4: return launch_g<Fixed3Engine<4, EX>, GeomStream>(A, P, grid, st);
+	case 5: case 6: return launch_g<Fixed3Engine<6, EX>, GeomStream>(A, P, grid, st);
+	default: return launch_g<Fixed3Engine<8, EX>, GeomStream>(A, P, grid, st);
 	}
 }
 
 template <int D, bool AL>
-static cudaError_t launch_fixedb_k(const ScanArgs &A, const FixedParams &P, int grid, cudaStream_t st)
+static cudaError_t launch_balanced(const ScanArgs &A, const FixedParams &P, int grid, cudaStream_t st)
 {
 	switch (P.ntests) {
 	case 2: return launch_g<FixedBEngine<D, 2, AL>, GeomPair>(A, P, grid, st);
@@ -1373,65 +1334,49 @@ static cudaError_t launch_fixedb_k(const ScanArgs &A, const FixedParams &P, int 
 	default: return launch_g<FixedBEngine<D, 8, AL>, GeomPair>(A, P, grid, st);
 	}
 }
-template <int D>
-static cudaError_t launch_fixedb(const ScanArgs &A, const FixedParams &P, int grid, cudaStream_t st)
-{
-	return P.b_aligned ? launch_fixedb_k<D, true>(A, P, grid, st) : launch_fixedb_k<D, false>(A, P, grid, st);
-}
-
-cudaError_t launch_scan_fixed(const ScanArgs &A, const FixedParams &P, int delta, const ScanGeom &g, int grid, cudaStream_t st)
-{
-	if (P.b_engine) {
-		switch (delta) {
-		case 1: return launch_fixedb<1>(A, P, grid, st);
-		case 2: return launch_fixedb<2>(A, P, grid, st);
-		case 3: return launch_fixedb<3>(A, P, grid, st);
-		default: return launch_fixedb<4>(A, P, grid, st);
-		}
-	}
-	if (P.stage1_triples) return P.exact3 ? launch_fixed3<true>(A, P, g, grid, st) : launch_fixed3<false>(A, P, g, grid, st);
-	const bool ex = P.exact != 0;
-	switch (delta) {
-	case 0: return ex ? launch_fixed_de<0, true>(A, P, g, grid, st) : launch_fixed_de<0, false>(A, P, g, grid, st);
-	case 1: return ex ? launch_fixed_de<1, true>(A, P, g, grid, st) : launch_fixed_de<1, false>(A, P, g, grid, st);
-	case 2: return ex ? launch_fixed_de<2, true>(A, P, g, grid, st) : launch_fixed_de<2, false>(A, P, g, grid, st);
-	case 3: return ex ? launch_fixed_de<3, true>(A, P, g, grid, st) : launch_fixed_de<3, false>(A, P, g, grid, st);
-	default: return ex ? launch_fixed_de<4, true>(A, P, g, grid, st) : launch_fixed_de<4, false>(A, P, g, grid, st);
-	}
-}
-
-#ifndef GS_RUN_STREAM
-#define GS_RUN_STREAM 0
-#endif
-constexpr bool kRunStream = GS_RUN_STREAM != 0; // RUN on the 4 KiB-slice geometry (tuning switch)
 
 template <int NHI, int NFO>
-static cudaError_t launch_run_hf(const ScanArgs &A, const RunParams &P, const ScanGeom &g, int grid, cudaStream_t st)
+static cudaError_t launch_run(const ScanArgs &A, const RunParams &P, int grid, cudaStream_t st)
 {
 	switch (P.nlo) {
-	case 0: case 1: return launch<RunEngine<1, NHI, NFO>, kRunStream>(A, P, g, grid, st);
-	case 2: return launch<RunEngine<2, NHI, NFO>, kRunStream>(A, P, g, grid, st);
-	case 3: return launch<RunEngine<3, NHI, NFO>, kRunStream>(A, P, g, grid, st);
-	case 4: return launch<RunEngine<4, NHI, NFO>, kRunStream>(A, P, g, grid, st);
-	case 5: case 6: return launch<RunEngine<6, NHI, NFO>, kRunStream>(A, P, g, grid, st);
-	default: return launch<RunEngine<8, NHI, NFO>, kRunStream>(A, P, g, grid, st);
+	case 0: case 1: return launch_g<RunEngine<1, NHI, NFO>, GeomBalanced>(A, P, grid, st);
+	case 2: return launch_g<RunEngine<2, NHI, NFO>, GeomBalanced>(A, P, grid, st);
+	case 3: return launch_g<RunEngine<3, NHI, NFO>, GeomBalanced>(A, P, grid, st);
+	case 4: return launch_g<RunEngine<4, NHI, NFO>, GeomBalanced>(A, P, grid, st);
+	case 5: case 6: return launch_g<RunEngine<6, NHI, NFO>, GeomBalanced>(A, P, grid, st);
+	default: return launch_g<RunEngine<8, NHI, NFO>, GeomBalanced>(A, P, grid, st);
 	}
 }
 
-cudaError_t launch_scan_run(const ScanArgs &A, const RunParams &P, const ScanGeom &g, int grid, cudaStream_t st)
+cudaError_t launch_scan(int kernel, const ScanArgs &A, const FixedParams &F, const HashParams &H, const RunParams &R, int delta,
+                        int grid, cudaStream_t st)
 {
-	if (P.nfold) {
-		switch (P.nhi) {
-		case 0: return launch_run_hf<0, 1>(A, P, g, grid, st);
-		case 1: return launch_run_hf<1, 1>(A, P, g, grid, st);
-		default: return launch_run_hf<2, 1>(A, P, g, grid, st);
+	switch (kernel) {
+	case GSCAN_KERNEL_PAIR:
+		switch (delta) {
+		case 0: return launch_pair<0, false>(A, F, grid, st); // a single-byte filter is never exact (gscan_compile)
+		case 1: return F.exact ? launch_pair<1, true>(A, F, grid, st) : launch_pair<1, false>(A, F, grid, st);
+		case 2: return F.exact ? launch_pair<2, true>(A, F, grid, st) : launch_pair<2, false>(A, F, grid, st);
+		case 3: return F.exact ? launch_pair<3, true>(A, F, grid, st) : launch_pair<3, false>(A, F, grid, st);
+		default: return F.exact ? launch_pair<4, true>(A, F, grid, st) : launch_pair<4, false>(A, F, grid, st);
+		}
+	case GSCAN_KERNEL_TRIPLE: return F.exact3 ? launch_triple<true>(A, F, grid, st) : launch_triple<false>(A, F, grid, st);
+	case GSCAN_KERNEL_BALANCED:
+		switch (delta) {
+		case 1: return F.b_aligned ? launch_balanced<1, true>(A, F, grid, st) : launch_balanced<1, false>(A, F, grid, st);
+		case 2: return F.b_aligned ? launch_balanced<2, true>(A, F, grid, st) : launch_balanced<2, false>(A, F, grid, st);
+		case 3: return F.b_aligned ? launch_balanced<3, true>(A, F, grid, st) : launch_balanced<3, false>(A, F, grid, st);
+		default: return F.b_aligned ? launch_balanced<4, true>(A, F, grid, st) : launch_balanced<4, false>(A, F, grid, st);
+		}
+	case GSCAN_KERNEL_HASH: return launch_g<HashEngine, GeomHash>(A, H, grid, st);
+	case GSCAN_KERNEL_RUN:
+		switch (R.nhi) {
+		case 0: return R.nfold ? launch_run<0, 1>(A, R, grid, st) : launch_run<0, 0>(A, R, grid, st);
+		case 1: return R.nfold ? launch_run<1, 1>(A, R, grid, st) : launch_run<1, 0>(A, R, grid, st);
+		default: return R.nfold ? launch_run<2, 1>(A, R, grid, st) : launch_run<2, 0>(A, R, grid, st);
 		}
 	}
-	switch (P.nhi) {
-	case 0: return launch_run_hf<0, 0>(A, P, g, grid, st);
-	case 1: return launch_run_hf<1, 0>(A, P, g, grid, st);
-	default: return launch_run_hf<2, 0>(A, P, g, grid, st);
-	}
+	return cudaErrorInvalidValue; // GSCAN_KERNEL_NONE: the pattern has no scan kernel
 }
 
 } // namespace gscan

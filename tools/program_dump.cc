@@ -16,7 +16,7 @@ int main(int argc, char **argv) {
 		for (auto &t : p.tests) mix(&t, sizeof t);
 		mix(&p.anchor, 4); mix(&p.delta, 4); mix(&p.delta2, 4);
 		for (auto &t : p.triples) mix(&t, sizeof t);
-		bool b1 = p.stage1_triples, b2 = p.disjoint, b3 = p.use_hash, b4 = p.use_vm, b5 = p.vm_runstart; mix(&b1,1); mix(&b2,1); mix(&b3,1); mix(&b4,1); mix(&b5,1);
+		bool b2 = p.disjoint, b3 = p.use_hash, b4 = p.use_vm, b5 = p.vm_runstart; mix(&p.pair_flag_prior, 8); mix(&b2,1); mix(&b3,1); mix(&b4,1); mix(&b5,1);
 		mix(&p.hash_len, 4); mix(&p.hash_mul, 4); mix(&p.hash_slots, 4);
 		if (!p.hash_table.empty()) mix(p.hash_table.data(), p.hash_table.size() * 4);
 		if (!p.slot_seqs.empty()) mix(p.slot_seqs.data(), p.slot_seqs.size() * 4);
